@@ -421,7 +421,9 @@ static bool inline_loops() {
     }                                     \
   } while (0)
 // P-384 keeps its call-based field operations in FOR_CURVE_INL: the all-inlined 12-limb fixed-base kernel under its
-// 128-register bound returns wrong points when built for sm_90a (tests/test_gpu_p384.py::test_golden_vectors).
+// 128-register bound returns wrong points when built for sm_90a by nvcc 12.9 (scalars near n among them), while its
+// field policy and point formulas are right under the same bound (DESIGN.md section 4;
+// tests/test_gpu_field_layer.py::test_fixedbase_p384_all_inlined keeps the reproducer).
 #define FOR_CURVE(curve, ...)             \
   do {                                    \
     if ((curve) == ECG_SECP256K1) {       \
