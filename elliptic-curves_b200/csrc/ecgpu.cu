@@ -11,17 +11,27 @@
 #include <string>
 #include <vector>
 
-// This file is compiled once per curve group (-DECG_TU=0..3) so that the groups build in parallel and the kernels of
+// This file is compiled once per curve group (-DECG_TU=0..5) so that the groups build in parallel and the kernels of
 // the headline curves keep their own translation unit:
 //   ECG_TU 0: secp256k1, P-256, P-384 + every extern "C" entry (entries for other curves forward to their group)
 //   ECG_TU 1: sm2, brainpoolP256r1/t1, bign-curve256v1 (8 limbs)   ECG_TU 2: brainpoolP384r1/t1 (12 limbs)
 //   ECG_TU 3: P-224 (7 limbs), P-192 (6 limbs)                    ECG_TU 4: P-521 (17 limbs, 66-byte records)
+//   ECG_TU 5: X448 (Curve448, 14 limbs, 56-byte records): the host pipeline and the ladder kernel, no Weierstrass code
 // The groups 1-3 run the generic kernels over the generic Montgomery field policy (ecg_fe_mont.cuh).
 #ifndef ECG_TU
 #define ECG_TU 0
 #endif
 
 #include "../../include/ecgpu.h"
+#if ECG_TU == 5
+#include "ecg_x448.cuh"
+using namespace ecg;
+// the status flags of ecg_kernels.cuh that finish() reads; every 56-byte string is a valid X448 input, so the X448
+// kernel reports none
+#define ERRF_SCALAR 1u
+#define ERRF_POINT 2u
+#define ERRF_SKEW 4u
+#else
 #include "ecg_kernels.cuh"
 #if ECG_TU == 0 || ECG_TU == 4  // hash to curve: secp256k1, P-256, P-384 (group 0) and P-521 (group 4)
 #include "ecg_h2c.cuh"
@@ -30,6 +40,7 @@
 #include "ecg_microbench.cuh"
 #endif
 #include "ecg_msm.cuh"
+#endif
 
 #define ECG_CURVE_COUNT 12
 static inline int curve_group(int c) { return c <= 2 ? 0 : c <= 6 ? 1 : c <= 8 ? 2 : c <= 10 ? 3 : 4; }
@@ -395,6 +406,7 @@ static void identity_xyz(uint8_t* z, ecg_curve c) {
   memset(z, 0, 3 * fb);
   z[curve_le(c) ? fb : 2 * fb - 1] = 1;
 }
+#if ECG_TU != 5  // the Weierstrass curves: kernels, fixed-base tables and the per-element batch driver
 // ECG_INLINE_LOOPS=0 (environment) keeps the call-based field operations in the one-point-operation-per-iteration
 // kernels (fixed-base, bucket accumulation): measurement knob, default = inlined
 static bool inline_loops() {
@@ -988,6 +1000,7 @@ static ecg_status run_chunk(ecg_ctx* ctx, DevState& d, Lane& L, const BatchOp& o
   if (op.kind != BatchOp::FIELD) ST_TRY(launch_norm(ctx, d, L, op.curve, cnt, jac, dp.out, dp.oinf, op.x_only));
   return copy_back(ctx, L, off, cnt, op.out, op.ostride, op.oinf, dp);
 }
+#endif  // ECG_TU != 5
 
 // Chunks of one device's range in host-pointer mode.  Two things cost time when a batch is cut into chunks: the first
 // chunk's upload and the last chunk's download are not hidden behind a kernel of the other lane, and every chunk whose
@@ -1013,6 +1026,7 @@ static std::vector<Shard> chunk_schedule(size_t cnt, size_t wave) {
   return v;
 }
 
+#if ECG_TU != 5
 static ecg_status run_batch_inner(ecg_ctx* ctx, const BatchOp& op, size_t n) {
   std::vector<Shard> shards = make_shards(n, ctx->devs.size());
   bool need_table = (op.kind == BatchOp::MULGEN && !(ctx->flags & ECG_FLAG_CONSTTIME)) || op.kind == BatchOp::MULGENADD ||
@@ -2129,3 +2143,64 @@ extern "C" ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double*
   return ECG_OK;
 }
 #endif  // ECG_TU == 0
+#endif  // ECG_TU != 5
+
+// ---- X448 (ecg_x448.cuh): group 5 holds the kernel; the public symbol (group 0) forwards there -------------------------
+#if ECG_TU == 0
+__attribute__((visibility("hidden"))) ecg_status ecg_tu5_ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56,
+                                                                         uint8_t* ok);
+extern "C" ecg_status ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok) {
+  return ecg_tu5_ecg_x448_batch(ctx, n, k56, u56, out56, ok);
+}
+#elif ECG_TU == 5
+// one chunk: stage the scalars and u values, one ladder per thread, copy the results and the low-order flags back
+static ecg_status x448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, const uint8_t* k56, const uint8_t* u56, uint8_t* out56,
+                             uint8_t* ok) {
+  DevPtrs dp;
+  ST_TRY(begin_lane(ctx, L));
+  ST_TRY(stage_in(ctx, L, B_K, k56, off, cnt, 56, &dp.k));
+  ST_TRY(stage_in(ctx, L, B_P, u56, off, cnt, 56, &dp.p));
+  ST_TRY(stage_out(ctx, L, off, cnt, out56, 56, ok, dp));
+  DOM_BEGIN(ctx, L);
+  x448_kernel<FpP448, X448_BLOCK, X448_MINBLK><<<grid_for(cnt, X448_BLOCK), X448_BLOCK, 0, L.s()>>>(dp.k, dp.p, cnt, dp.out, dp.oinf);
+  LAUNCHED(ctx);
+  DOM_END(ctx, L);
+  return copy_back(ctx, L, off, cnt, out56, 56, ok, dp);
+}
+// the batch split of run_batch_inner: device-pointer mode in DEV_CHUNK pieces on lane 0; host mode sharded over the
+// devices and cut into whole waves of the ladder kernel, alternating lanes so that copies overlap the kernels
+static ecg_status x448_run(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok) {
+  if (ctx->devptr()) {
+    DevState& d = ctx->devs[0];
+    CU_TRY(ctx, cudaSetDevice(d.dev));
+    for (size_t lo = 0; lo < n; lo += DEV_CHUNK) ST_TRY(x448_chunk(ctx, d.lane[0], lo, std::min(DEV_CHUNK, n - lo), k56, u56, out56, ok));
+    return finish(ctx);
+  }
+  std::vector<Shard> shards = make_shards(n, ctx->devs.size());
+  std::vector<std::vector<Shard>> sched(shards.size());
+  size_t maxchunks = 0;
+  for (size_t i = 0; i < shards.size(); i++) {
+    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * X448_MINBLK * X448_BLOCK);
+    maxchunks = std::max(maxchunks, sched[i].size());
+  }
+  for (size_t c = 0; c < maxchunks; c++) {
+    for (size_t i = 0; i < ctx->devs.size(); i++) {
+      if (c >= sched[i].size()) continue;
+      DevState& d = ctx->devs[i];
+      CU_TRY(ctx, cudaSetDevice(d.dev));
+      ST_TRY(x448_chunk(ctx, d.lane[c & 1], shards[i].off + sched[i][c].off, sched[i][c].cnt, k56, u56, out56, ok));
+    }
+  }
+  return finish(ctx);
+}
+ECG_API(ecg_x448_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok) {
+  if (!ctx) return ECG_EINVAL;
+  if (n == 0) return ECG_OK;
+  if (!k56 || !out56) {
+    ctx->err = "ecg_x448_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = x448_run(ctx, n, k56, u56, out56, ok);
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+#endif

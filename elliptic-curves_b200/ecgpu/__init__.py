@@ -9,6 +9,7 @@ bench.py.  It mirrors the reference's names for the hot path:
     Engine.mul_by_generator_and_mul_add(...)   MulByGeneratorVartime::..._and_mul_add    (mul.rs:303-310)
     Engine.batch_normalize(curve, XYZ)         BatchNormalize::batch_normalize           (projective.rs:345-391)
     Engine.field_op(curve, op, a, b)           FieldElement add/sub/neg/mul/square/invert
+    Engine.x448(k56, u56)                      x448::x448_unchecked / EphemeralSecret::diffie_hellman (x448/src/lib.rs)
 
 Buffers are numpy uint8 arrays (host mode) or raw device pointers (device mode, ECG_FLAG_DEVICE_PTRS).
 There is NO CPU fallback: if libecgpu.so is missing, or no CUDA device is present, construction raises.
@@ -53,6 +54,7 @@ EXPORTS = [
     "ecg_schnorr_verify_batch", "ecg_ecdsa_verify_batch", "ecg_decompress_batch",
     "ecg_batch_normalize_hom", "ecg_mul_batch_x", "ecg_field_sqrt_batch",
     "ecg_hash_to_curve_batch", "ecg_hash_to_scalar_batch", "ecg_sm2dsa_verify_batch", "ecg_ecdsa_recover_batch",
+    "ecg_x448_batch",
 ]
 
 
@@ -138,6 +140,8 @@ def load_library(path: Optional[str] = None) -> ctypes.CDLL:
     lib.ecg_hash_to_curve_batch.restype = ctypes.c_int
     lib.ecg_hash_to_scalar_batch.argtypes = [vp, ctypes.c_int, sz, u8p, u8p, u8p, sz, u8p]
     lib.ecg_hash_to_scalar_batch.restype = ctypes.c_int
+    lib.ecg_x448_batch.argtypes = [vp, sz, u8p, u8p, u8p, u8p]
+    lib.ecg_x448_batch.restype = ctypes.c_int
     lib.ecg_version.argtypes = []
     lib.ecg_version.restype = ctypes.c_char_p
     if path is None:
@@ -507,6 +511,20 @@ class Engine:
         self._check(self.lib.ecg_field_op_batch(self._ctx, c, FOP[op] if isinstance(op, str) else op, n, _ptr(a), _ptr(b), _ptr(out)))
         return out.reshape(n, fb)
 
+    def x448(self, k56, u56=None, out=None, ok=None):
+        """X448 (RFC 7748) over a batch -> (out n x 56, ok n): out[i] = X448(k[i], u[i]) (x448::x448_unchecked); u56=None:
+        u = 5, the public keys of the secrets (PublicKey::from).  ok[i] = 0 iff u[i] is byte-for-byte one of the
+        low-order encodings x448::x448 refuses.  An all-zero out[i] (RFC 7748 section 6.2) is not refused here: compare
+        with zero bytes where the protocol asks for it."""
+        n = np.asarray(k56).size // 56
+        k56 = _u8(k56, 56 * n, "k56")
+        if u56 is not None:
+            u56 = _u8(u56, 56 * n, "u56")
+        out = _out(out, 56 * n, "out")
+        ok = _out(ok, n, "ok")
+        self._check(self.lib.ecg_x448_batch(self._ctx, n, _ptr(k56), _ptr(u56), _ptr(out), _ptr(ok)))
+        return out.reshape(n, 56), ok
+
     # ---- raw-pointer API (device_ptrs=True): all arguments are integer CUDA device addresses ----
     def mul_batch_ptr(self, curve, n, k, P_xy, P_inf, out_xy, out_inf):
         self._check(self.lib.ecg_mul_batch(self._ctx, CURVE_IDS[curve], n, _ptr(k), _ptr(P_xy), _ptr(P_inf), _ptr(out_xy), _ptr(out_inf)))
@@ -526,6 +544,10 @@ class Engine:
 
     def schnorr_verify_ptr(self, n, pk_x, msg32, sig64, valid):
         self._check(self.lib.ecg_schnorr_verify_batch(self._ctx, n, _ptr(pk_x), _ptr(msg32), _ptr(sig64), _ptr(valid)))
+
+    def x448_ptr(self, n, k56, u56, out56, ok):
+        """ecg_x448_batch on device buffers (u56 = 0: the generator; ok = 0: no flags)"""
+        self._check(self.lib.ecg_x448_batch(self._ctx, n, _ptr(k56), _ptr(u56), _ptr(out56), _ptr(ok)))
 
     def timing_enable(self, on: bool = True):
         self._check(self.lib.ecg_timing_enable(self._ctx, 1 if on else 0))

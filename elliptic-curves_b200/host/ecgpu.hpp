@@ -11,6 +11,7 @@
 //   Engine::batch_normalize(jacobian)                 <->  BatchNormalize::batch_normalize     (projective.rs:345-365)
 //   Engine::hash_to_curve / encode_to_curve / hash_to_scalar <-> GroupDigest::hash_from_bytes / encode_from_bytes,
 //                                                         hash2curve::hash_to_scalar (hash2curve/src/group_digest.rs:88-143)
+//   Engine::x448(k, u)                                <->  x448::x448_unchecked / EphemeralSecret::diffie_hellman (x448/src/lib.rs)
 // The typed surface below is for the 256-bit curves with big-endian records (secp256k1, P-256, sm2, brainpoolP256r1/t1);
 // the other curves of include/ecgpu.h (48 / 28 / 24-byte records, bign's little-endian records) are reached through the
 // C ABI directly or the Python mirror, which sizes its buffers per curve.
@@ -126,6 +127,23 @@ class Engine {
     std::vector<uint8_t> sq(n);
     check(ecg_field_sqrt_batch(ctx_, curve_, n, reinterpret_cast<const uint8_t*>(a.data()), reinterpret_cast<uint8_t*>(r.data()), sq.data()));
     if (ok) ok->assign(sq.begin(), sq.end());
+    return r;
+  }
+
+  // ---- X448 (RFC 7748), 56-byte little-endian records; the same on an Engine of any curve ----
+  using X448Bytes = std::array<uint8_t, 56>;
+  // x448::x448_unchecked / EphemeralSecret::diffie_hellman over a batch (x448/src/lib.rs:25-31, :159-163); u empty: u = 5
+  // for every scalar, the public keys (PublicKey::from).  ok (optional): ok[i] = false where u[i] is byte-for-byte one of
+  // the low-order encodings x448::x448 refuses.  An all-zero result is returned, not refused (RFC 7748 section 6.2 leaves
+  // that check to the protocol).
+  std::vector<X448Bytes> x448(const std::vector<X448Bytes>& k, const std::vector<X448Bytes>& u = {}, std::vector<bool>* ok = nullptr) {
+    size_t n = k.size();
+    if (!u.empty()) check_sizes(n, u.size());
+    std::vector<X448Bytes> r(n);
+    std::vector<uint8_t> flags(n);
+    check(ecg_x448_batch(ctx_, n, reinterpret_cast<const uint8_t*>(k.data()), u.empty() ? nullptr : reinterpret_cast<const uint8_t*>(u.data()),
+                         reinterpret_cast<uint8_t*>(r.data()), flags.data()));
+    if (ok) ok->assign(flags.begin(), flags.end());
     return r;
   }
 

@@ -1,5 +1,5 @@
 /* ecgpu.h — C ABI of libecgpu.so: H100-native batched elliptic-curve scalar multiplication
- * (secp256k1 / NIST P-256).
+ * (secp256k1 / NIST P-256 on the hot path, every prime-order Weierstrass curve of the reference, and X448 key exchange).
  *
  * The reference (RustCrypto/elliptic-curves @ 739304e) has NO FFI boundary; its seams are Rust traits.
  * Each entry point below names the trait method(s) / function(s) it stands in for (paths relative to the
@@ -259,6 +259,24 @@ ecg_status ecg_hash_to_scalar_batch(ecg_ctx* ctx, ecg_curve curve, size_t n, con
 ecg_status ecg_field_op_batch(ecg_ctx* ctx, ecg_curve curve, int op, size_t n, const uint8_t* a,
                               const uint8_t* b, uint8_t* out);
 
+/* ---- X448 (RFC 7748): Diffie-Hellman on Curve448 -----------------------------------------------------------------
+ * Curve448 is a Montgomery curve, not one of the Weierstrass curves above, so this entry takes no ecg_curve.  Records are
+ * 56 bytes, little-endian, as in the RFC; every 56-byte string is a valid input.
+ * out56[i] = X448(k56[i], u56[i]) (RFC 7748) — x448::x448_unchecked / EphemeralSecret::diffie_hellman over a batch
+ * (x448/src/lib.rs:25-31, :159-163): the scalar is clamped (k[0] &= 252, k[55] |= 128) and used without reduction mod
+ * the group order; u is reduced mod p = 2^448 - 2^224 - 1; the result is canonical, 56 zero bytes at the identity.
+ * u56 == NULL: u = 5 for every i (PublicKey::from(&EphemeralSecret), x448/src/lib.rs:109-114).  ok[i] (may be NULL) = 0
+ * iff u56[i] is byte-for-byte one of the three low-order encodings x448::x448 refuses (0, 1, p - 1:
+ * MontgomeryPoint::LOW_A / LOW_B / LOW_C, ed448-goldilocks/src/montgomery.rs:22-42), else 1; out56[i] is computed
+ * either way.  Like the reference, the entry does not refuse an all-zero shared secret (RFC 7748 section 6.2): a caller
+ * that needs the check compares out56[i] with 56 zero bytes.
+ * Errors: ECG_EINVAL (null ctx, or null k56 / out56 with n > 0) and CUDA errors; n = 0 is ECG_OK.  With
+ * ECG_FLAG_DEVICE_PTRS all four arrays are device pointers (the 56-byte records 4-byte aligned).  ECG_FLAG_ZEROIZE scrubs
+ * the staged scalars, u values, results and flags on the device.  ECG_FLAG_CONSTTIME is accepted and changes nothing:
+ * the ladder is constant time in every mode (masked conditional swaps, a fixed inversion chain, no table, no branch
+ * on the scalar or on u). */
+ecg_status ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok);
+
 /* ---- measurement helpers (not part of the reference-facing surface) ---- */
 
 /* Integer-pipe microbenchmark on device 0 of the ctx: which = 0 IMAD.WIDE.U32.X carry chains (the
@@ -267,7 +285,7 @@ ecg_status ecg_field_op_batch(ecg_ctx* ctx, ecg_curve curve, int op, size_t n, c
  * of the named kind, or field multiplications for 3/4). */
 ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double* ops_per_s, double* elapsed_ms);
 
-/* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication)
+/* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication, the X448 ladder)
  * with CUDA events on the launching stream; ecg_timing_read returns the accumulated device milliseconds
  * (max over the ctx's devices per call) and the number of calls since ecg_timing_enable. */
 ecg_status ecg_timing_enable(ecg_ctx* ctx, int on);

@@ -86,6 +86,9 @@ unsafe extern "C" {
     /// `AffinePoint::decompress` over a batch (primeorder/src/affine.rs:179-198)
     pub fn ecg_decompress_batch(ctx: *mut ecg_ctx, curve: i32, n: usize, sec1_33: *const u8, out_xy: *mut u8,
                                 out_inf: *mut u8, valid: *mut u8) -> i32;
+    /// X448 (RFC 7748) over a batch: `x448::x448_unchecked` / `EphemeralSecret::diffie_hellman` (x448/src/lib.rs:25-31,
+    /// :159-163); `u56` null: u = 5 (`PublicKey::from`); `ok` (may be null): 0 where `x448::x448` returns `None`
+    pub fn ecg_x448_batch(ctx: *mut ecg_ctx, n: usize, k56: *const u8, u56: *const u8, out56: *mut u8, ok: *mut u8) -> i32;
     pub fn ecg_kernel_launches(ctx: *const ecg_ctx) -> u64;
 }
 
@@ -124,6 +127,21 @@ impl GpuEngine {
             ECG_OK => Ok(Self { ctx, curve }),
             _ => Err(GpuError::Cuda("ecg_ctx_create failed: no CUDA device (there is no CPU fallback)".into())),
         }
+    }
+
+    /// X448 over a batch, for an engine of any curve.  `u: None`: the public keys of the secrets `k` (`PublicKey::from`).
+    /// Returns `(out, ok)`: `out[i] = x448::x448_unchecked(k[i], u[i])`, and `ok[i] = false` where `x448::x448(k[i], u[i])`
+    /// is `None` (u is byte-for-byte a low-order encoding), so `x448::x448` is `ok[i].then_some(out[i])`.
+    pub fn batch_x448(&mut self, k: &[[u8; 56]], u: Option<&[[u8; 56]]>) -> Result<(Vec<[u8; 56]>, Vec<bool>), GpuError> {
+        let n = k.len();
+        if let Some(u) = u {
+            assert!(u.len() == n);
+        }
+        let (mut out, mut ok) = (vec![[0u8; 56]; n], vec![0u8; n]);
+        let u_ptr = u.map_or(core::ptr::null(), |u| u.as_ptr().cast());
+        // SAFETY: k, u (when given), out hold n 56-byte records, ok n bytes.
+        let rc = unsafe { ecg_x448_batch(self.ctx, n, k.as_ptr().cast(), u_ptr, out.as_mut_ptr().cast(), ok.as_mut_ptr()) };
+        self.check(rc).map(|_| (out, ok.into_iter().map(|b| b != 0).collect()))
     }
 
     /// `out[i] = k[i] * P[i]` — batch form of `Mul<Scalar> for ProjectivePoint` / `MulVartime`.

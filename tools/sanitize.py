@@ -66,6 +66,15 @@ def main():
         pk[i] = np.frombuffer(px, np.uint8); sg[i] = np.frombuffer(s64, np.uint8)
         assert pyref.bip340_verify(px, msg[i].tobytes(), s64)
     assert eng.schnorr_verify_batch(pk, msg, sg).all()
+    # X448: a few pairs, low-order encodings among them, and the generator form
+    import x448_model
+    k448 = [os.urandom(56) for _ in range(16)]
+    u448 = list(x448_model.LOW_ORDER) + [os.urandom(56) for _ in range(13)]
+    out, ok = eng.x448(np.frombuffer(b"".join(k448), np.uint8), np.frombuffer(b"".join(u448), np.uint8))
+    for i in range(16):
+        assert out[i].tobytes() == x448_model.x448(k448[i], u448[i]) and ok[i] == x448_model.u_ok(u448[i]), ("x448", i)
+    pub, _ = eng.x448(np.frombuffer(b"".join(k448[:4]), np.uint8))
+    assert pub[0].tobytes() == x448_model.x448(k448[0], x448_model.GENERATOR)
     eng.close()
     print("sanitize workload OK")
 
