@@ -11,23 +11,28 @@
 #include <string>
 #include <vector>
 
-// This file is compiled once per curve group (-DECG_TU=0..5) so that the groups build in parallel and the kernels of
+// This file is compiled once per curve group (-DECG_TU=0..6) so that the groups build in parallel and the kernels of
 // the headline curves keep their own translation unit:
 //   ECG_TU 0: secp256k1, P-256, P-384 + every extern "C" entry (entries for other curves forward to their group)
 //   ECG_TU 1: sm2, brainpoolP256r1/t1, bign-curve256v1 (8 limbs)   ECG_TU 2: brainpoolP384r1/t1 (12 limbs)
 //   ECG_TU 3: P-224 (7 limbs), P-192 (6 limbs)                    ECG_TU 4: P-521 (17 limbs, 66-byte records)
 //   ECG_TU 5: X448 (Curve448, 14 limbs, 56-byte records): the host pipeline and the ladder kernel, no Weierstrass code
+//   ECG_TU 6: Ed448 verification (the Edwards group on the Curve448 field, SHAKE256): the host pipeline and its kernel
 // The groups 1-3 run the generic kernels over the generic Montgomery field policy (ecg_fe_mont.cuh).
 #ifndef ECG_TU
 #define ECG_TU 0
 #endif
 
 #include "../../include/ecgpu.h"
+#if ECG_TU == 5 || ECG_TU == 6
 #if ECG_TU == 5
 #include "ecg_x448.cuh"
+#else
+#include "ecg_ed448.cuh"
+#endif
 using namespace ecg;
-// the status flags of ecg_kernels.cuh that finish() reads; every 56-byte string is a valid X448 input, so the X448
-// kernel reports none
+// the status flags of ecg_kernels.cuh that finish() reads; every 56-byte string is a valid X448 input, and an Ed448
+// encoding that does not decode is a verdict (valid = 0), so neither kernel reports any
 #define ERRF_SCALAR 1u
 #define ERRF_POINT 2u
 #define ERRF_SKEW 4u
@@ -406,7 +411,7 @@ static void identity_xyz(uint8_t* z, ecg_curve c) {
   memset(z, 0, 3 * fb);
   z[curve_le(c) ? fb : 2 * fb - 1] = 1;
 }
-#if ECG_TU != 5  // the Weierstrass curves: kernels, fixed-base tables and the per-element batch driver
+#if ECG_TU < 5  // the Weierstrass curves: kernels, fixed-base tables and the per-element batch driver
 // ECG_INLINE_LOOPS=0 (environment) keeps the call-based field operations in the one-point-operation-per-iteration
 // kernels (fixed-base, bucket accumulation): measurement knob, default = inlined
 static bool inline_loops() {
@@ -1000,7 +1005,7 @@ static ecg_status run_chunk(ecg_ctx* ctx, DevState& d, Lane& L, const BatchOp& o
   if (op.kind != BatchOp::FIELD) ST_TRY(launch_norm(ctx, d, L, op.curve, cnt, jac, dp.out, dp.oinf, op.x_only));
   return copy_back(ctx, L, off, cnt, op.out, op.ostride, op.oinf, dp);
 }
-#endif  // ECG_TU != 5
+#endif  // ECG_TU < 5
 
 // Chunks of one device's range in host-pointer mode.  Two things cost time when a batch is cut into chunks: the first
 // chunk's upload and the last chunk's download are not hidden behind a kernel of the other lane, and every chunk whose
@@ -1026,7 +1031,7 @@ static std::vector<Shard> chunk_schedule(size_t cnt, size_t wave) {
   return v;
 }
 
-#if ECG_TU != 5
+#if ECG_TU < 5
 static ecg_status run_batch_inner(ecg_ctx* ctx, const BatchOp& op, size_t n) {
   std::vector<Shard> shards = make_shards(n, ctx->devs.size());
   bool need_table = (op.kind == BatchOp::MULGEN && !(ctx->flags & ECG_FLAG_CONSTTIME)) || op.kind == BatchOp::MULGENADD ||
@@ -2143,7 +2148,7 @@ extern "C" ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double*
   return ECG_OK;
 }
 #endif  // ECG_TU == 0
-#endif  // ECG_TU != 5
+#endif  // ECG_TU < 5
 
 // ---- X448 (ecg_x448.cuh): group 5 holds the kernel; the public symbol (group 0) forwards there -------------------------
 #if ECG_TU == 0
@@ -2201,6 +2206,126 @@ ECG_API(ecg_x448_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_
     return ECG_EINVAL;
   }
   ecg_status st = x448_run(ctx, n, k56, u56, out56, ok);
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+#endif
+
+// ---- Ed448 verification (ecg_ed448.cuh): group 6 holds the kernel; the public symbol (group 0) forwards there ----------
+#if ECG_TU == 0
+__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114,
+                                                                                 const uint8_t* msgs, const uint64_t* offsets, const uint8_t* context,
+                                                                                 size_t context_len, int prehashed, uint8_t* valid);
+extern "C" ecg_status ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs,
+                                             const uint64_t* offsets, const uint8_t* context, size_t context_len, int prehashed, uint8_t* valid) {
+  return ecg_tu6_ecg_ed448_verify_batch(ctx, n, pk57, sig114, msgs, offsets, context, context_len, prehashed, valid);
+}
+#elif ECG_TU == 6
+// one chunk [off, off + cnt): stage the keys, the signatures, the chunk's own byte range of the messages and its offsets
+// (the kernel subtracts the range's start), one verification per thread, copy the verdicts back
+static ecg_status ed448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs,
+                              const uint64_t* offsets, const Ed448Dom& dom, uint8_t* valid) {
+  DevPtrs dp;
+  ST_TRY(begin_lane(ctx, L));
+  ST_TRY(stage_in(ctx, L, B_K, pk57, off, cnt, 57, &dp.k));
+  ST_TRY(stage_in(ctx, L, B_P, sig114, off, cnt, 114, &dp.p));
+  const uint8_t* dmsgs = msgs;
+  const uint64_t* doffs = offsets + off;
+  uint64_t base = 0;
+  if (!ctx->devptr()) {
+    base = offsets[off];
+    const uint64_t total = offsets[off + cnt] - base;
+    ST_TRY(ensure(ctx, L, B_A, (size_t)total + 16));
+    ST_TRY(ensure(ctx, L, B_X, (cnt + 1) * 8));
+    if (total) CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_A], msgs + base, (size_t)total, cudaMemcpyHostToDevice, L.s()));
+    CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_X], offsets + off, (cnt + 1) * 8, cudaMemcpyHostToDevice, L.s()));
+    dmsgs = (const uint8_t*)L.buf[B_A];
+    doffs = (const uint64_t*)L.buf[B_X];
+  }
+  ST_TRY(stage_out(ctx, L, off, cnt, valid, 1, nullptr, dp));
+  DOM_BEGIN(ctx, L);
+  ed448_verify_kernel<FpEd448, ED448_BLOCK, ED448_MINBLK><<<grid_for(cnt, ED448_BLOCK), ED448_BLOCK, 0, L.s()>>>(dp.k, dp.p, dmsgs, doffs, base, cnt,
+                                                                                                              dom, dp.out);
+  LAUNCHED(ctx);
+  DOM_END(ctx, L);
+  return copy_back(ctx, L, off, cnt, valid, 1, nullptr, dp);
+}
+// offsets[0..n] must not decrease (in device-pointer mode they are read back first: 8 (n + 1) bytes)
+static ecg_status ed448_check_offsets(ecg_ctx* ctx, size_t n, const uint64_t* offsets, const uint8_t* msgs) {
+  std::vector<uint64_t> host;
+  const uint64_t* o = offsets;
+  if (ctx->devptr()) {
+    if (reinterpret_cast<uintptr_t>(offsets) & 7) {
+      ctx->err = "ecg_ed448_verify_batch: device pointer (offsets) not 8-byte aligned";
+      return ECG_EINVAL;
+    }
+    Lane& L = ctx->devs[0].lane[0];
+    host.resize(n + 1);
+    CU_TRY(ctx, cudaSetDevice(ctx->devs[0].dev));
+    CU_TRY(ctx, cudaMemcpyAsync(host.data(), offsets, (n + 1) * 8, cudaMemcpyDeviceToHost, L.s()));
+    CU_TRY(ctx, cudaStreamSynchronize(L.s()));
+    o = host.data();
+  }
+  for (size_t i = 0; i < n; i++)
+    if (o[i + 1] < o[i]) {
+      ctx->err = "ecg_ed448_verify_batch: message offsets must be non-decreasing";
+      return ECG_EINVAL;
+    }
+  if (!msgs && o[n] != o[0]) {
+    ctx->err = "ecg_ed448_verify_batch: null message buffer";
+    return ECG_EINVAL;
+  }
+  return ECG_OK;
+}
+// the batch split of x448_run: device-pointer mode in DEV_CHUNK pieces on lane 0; host mode sharded over the devices and
+// cut into whole waves of the kernel, alternating lanes so that copies overlap the kernels
+static ecg_status ed448_run(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs, const uint64_t* offsets,
+                            const Ed448Dom& dom, uint8_t* valid) {
+  if (ctx->devptr()) {
+    DevState& d = ctx->devs[0];
+    CU_TRY(ctx, cudaSetDevice(d.dev));
+    for (size_t lo = 0; lo < n; lo += DEV_CHUNK)
+      ST_TRY(ed448_chunk(ctx, d.lane[0], lo, std::min(DEV_CHUNK, n - lo), pk57, sig114, msgs, offsets, dom, valid));
+    return finish(ctx);
+  }
+  std::vector<Shard> shards = make_shards(n, ctx->devs.size());
+  std::vector<std::vector<Shard>> sched(shards.size());
+  size_t maxchunks = 0;
+  for (size_t i = 0; i < shards.size(); i++) {
+    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * ED448_MINBLK * ED448_BLOCK);
+    maxchunks = std::max(maxchunks, sched[i].size());
+  }
+  for (size_t c = 0; c < maxchunks; c++) {
+    for (size_t i = 0; i < ctx->devs.size(); i++) {
+      if (c >= sched[i].size()) continue;
+      DevState& d = ctx->devs[i];
+      CU_TRY(ctx, cudaSetDevice(d.dev));
+      ST_TRY(ed448_chunk(ctx, d.lane[c & 1], shards[i].off + sched[i][c].off, sched[i][c].cnt, pk57, sig114, msgs, offsets, dom, valid));
+    }
+  }
+  return finish(ctx);
+}
+ECG_API(ecg_ed448_verify_batch)(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs,
+                                const uint64_t* offsets, const uint8_t* context, size_t context_len, int prehashed, uint8_t* valid) {
+  if (!ctx) return ECG_EINVAL;
+  if (context_len > 255 || (context_len && !context)) {
+    ctx->err = "ecg_ed448_verify_batch: the context is at most 255 bytes";
+    return ECG_EINVAL;
+  }
+  if (n == 0) return ECG_OK;
+  if (!pk57 || !sig114 || !offsets || !valid) {
+    ctx->err = "ecg_ed448_verify_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = ed448_check_offsets(ctx, n, offsets, msgs);
+  if (st != ECG_OK) return st;
+  // dom4 = "SigEd448" || phflag || len(ctx) || ctx (RFC 8032 section 2; sign.rs:105, verifying_key.rs:290-303)
+  Ed448Dom dom;
+  memcpy(dom.b, "SigEd448", 8);
+  dom.b[8] = prehashed ? 1 : 0;
+  dom.b[9] = (uint8_t)context_len;
+  if (context_len) memcpy(dom.b + 10, context, context_len);
+  dom.len = (uint32_t)(10 + context_len);
+  st = ed448_run(ctx, n, pk57, sig114, msgs, offsets, dom, valid);
   return st == ECG_OK ? st : fail(ctx, st);
 }
 #endif

@@ -10,6 +10,7 @@ bench.py.  It mirrors the reference's names for the hot path:
     Engine.batch_normalize(curve, XYZ)         BatchNormalize::batch_normalize           (projective.rs:345-391)
     Engine.field_op(curve, op, a, b)           FieldElement add/sub/neg/mul/square/invert
     Engine.x448(k56, u56)                      x448::x448_unchecked / EphemeralSecret::diffie_hellman (x448/src/lib.rs)
+    Engine.ed448_verify(pk57, sig114, msgs)    ed448 VerifyingKey::verify_raw / verify_ctx / verify_prehashed
 
 Buffers are numpy uint8 arrays (host mode) or raw device pointers (device mode, ECG_FLAG_DEVICE_PTRS).
 There is NO CPU fallback: if libecgpu.so is missing, or no CUDA device is present, construction raises.
@@ -54,7 +55,7 @@ EXPORTS = [
     "ecg_schnorr_verify_batch", "ecg_ecdsa_verify_batch", "ecg_decompress_batch",
     "ecg_batch_normalize_hom", "ecg_mul_batch_x", "ecg_field_sqrt_batch",
     "ecg_hash_to_curve_batch", "ecg_hash_to_scalar_batch", "ecg_sm2dsa_verify_batch", "ecg_ecdsa_recover_batch",
-    "ecg_x448_batch",
+    "ecg_x448_batch", "ecg_ed448_verify_batch",
 ]
 
 
@@ -142,6 +143,8 @@ def load_library(path: Optional[str] = None) -> ctypes.CDLL:
     lib.ecg_hash_to_scalar_batch.restype = ctypes.c_int
     lib.ecg_x448_batch.argtypes = [vp, sz, u8p, u8p, u8p, u8p]
     lib.ecg_x448_batch.restype = ctypes.c_int
+    lib.ecg_ed448_verify_batch.argtypes = [vp, sz, u8p, u8p, u8p, u8p, u8p, sz, ctypes.c_int, u8p]
+    lib.ecg_ed448_verify_batch.restype = ctypes.c_int
     lib.ecg_version.argtypes = []
     lib.ecg_version.restype = ctypes.c_char_p
     if path is None:
@@ -525,6 +528,31 @@ class Engine:
         self._check(self.lib.ecg_x448_batch(self._ctx, n, _ptr(k56), _ptr(u56), _ptr(out), _ptr(ok)))
         return out.reshape(n, 56), ok
 
+    def ed448_verify(self, pk57, sig114, msgs, context: bytes = b"", prehashed: bool = False):
+        """Ed448 (RFC 8032) verification over a batch -> valid (n uint8): VerifyingKey::from_bytes(pk57[i]) and then
+        verify_ctx(sig114[i], context, msgs[i]) (verify_raw: context b""), or with prehashed=True verify_prehashed with
+        msgs[i] = PH(M) = SHAKE256(M, 64) as the caller computed it.  One context (<= 255 bytes) for the whole call."""
+        data, offs = self._pack_messages(msgs)
+        return self.ed448_verify_packed(pk57, sig114, data, offs, context, prehashed)
+
+    def ed448_verify_packed(self, pk57, sig114, data, offsets, context: bytes = b"", prehashed: bool = False, valid=None):
+        """the same over messages already laid out as the C ABI takes them: `data` = the messages back to back (uint8),
+        `offsets` = n + 1 uint64 byte offsets (message i = data[offsets[i]:offsets[i + 1]])"""
+        offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = offs.size - 1
+        if n < 0 or int(offs[-1]) > np.asarray(data).size:
+            raise ValueError("offsets: n + 1 ascending byte offsets into data")
+        data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+        if data.size == 0:
+            data = np.zeros(1, np.uint8)
+        pk57 = _u8(pk57, 57 * n, "pk57")
+        sig114 = _u8(sig114, 114 * n, "sig114")
+        ctx = np.frombuffer(bytes(context), np.uint8).copy() if len(context) else None
+        valid = _out(valid, n, "valid")
+        self._check(self.lib.ecg_ed448_verify_batch(self._ctx, n, _ptr(pk57), _ptr(sig114), _ptr(data), _ptr(offs), _ptr(ctx), len(context),
+                                                    1 if prehashed else 0, _ptr(valid)))
+        return valid
+
     # ---- raw-pointer API (device_ptrs=True): all arguments are integer CUDA device addresses ----
     def mul_batch_ptr(self, curve, n, k, P_xy, P_inf, out_xy, out_inf):
         self._check(self.lib.ecg_mul_batch(self._ctx, CURVE_IDS[curve], n, _ptr(k), _ptr(P_xy), _ptr(P_inf), _ptr(out_xy), _ptr(out_inf)))
@@ -548,6 +576,12 @@ class Engine:
     def x448_ptr(self, n, k56, u56, out56, ok):
         """ecg_x448_batch on device buffers (u56 = 0: the generator; ok = 0: no flags)"""
         self._check(self.lib.ecg_x448_batch(self._ctx, n, _ptr(k56), _ptr(u56), _ptr(out56), _ptr(ok)))
+
+    def ed448_verify_ptr(self, n, pk57, sig114, msgs, offsets, valid, context: bytes = b"", prehashed: bool = False):
+        """ecg_ed448_verify_batch on device buffers (offsets: n + 1 uint64, 8-byte aligned); the context is host bytes"""
+        ctx = np.frombuffer(bytes(context), np.uint8).copy() if len(context) else None
+        self._check(self.lib.ecg_ed448_verify_batch(self._ctx, n, _ptr(pk57), _ptr(sig114), _ptr(msgs), _ptr(offsets), _ptr(ctx), len(context),
+                                                    1 if prehashed else 0, _ptr(valid)))
 
     def timing_enable(self, on: bool = True):
         self._check(self.lib.ecg_timing_enable(self._ctx, 1 if on else 0))

@@ -12,6 +12,7 @@
 //   Engine::hash_to_curve / encode_to_curve / hash_to_scalar <-> GroupDigest::hash_from_bytes / encode_from_bytes,
 //                                                         hash2curve::hash_to_scalar (hash2curve/src/group_digest.rs:88-143)
 //   Engine::x448(k, u)                                <->  x448::x448_unchecked / EphemeralSecret::diffie_hellman (x448/src/lib.rs)
+//   Engine::ed448_verify(pk, sig, msgs, ctx, ph)      <->  ed448 VerifyingKey::verify_raw / verify_ctx / verify_prehashed
 // The typed surface below is for the 256-bit curves with big-endian records (secp256k1, P-256, sm2, brainpoolP256r1/t1);
 // the other curves of include/ecgpu.h (48 / 28 / 24-byte records, bign's little-endian records) are reached through the
 // C ABI directly or the Python mirror, which sizes its buffers per curve.
@@ -145,6 +146,30 @@ class Engine {
                          reinterpret_cast<uint8_t*>(r.data()), flags.data()));
     if (ok) ok->assign(flags.begin(), flags.end());
     return r;
+  }
+
+  // ---- Ed448 (RFC 8032) verification, 57-byte keys and 114-byte signatures; the same on an Engine of any curve ----
+  using Ed448Key = std::array<uint8_t, 57>;
+  using Ed448Sig = std::array<uint8_t, 114>;
+  // VerifyingKey::from_bytes(pk[i]) then verify_ctx(sig[i], context, msgs[i]) (verify_raw: empty context), or with
+  // prehashed = true verify_prehashed with msgs[i] = PH(M) = SHAKE256(M, 64) (ed448-goldilocks/src/sign/verifying_key.rs:
+  // 187-312); result[i] = true iff the reference accepts.  One context of at most 255 bytes for the whole call.
+  std::vector<bool> ed448_verify(const std::vector<Ed448Key>& pk, const std::vector<Ed448Sig>& sig, const std::vector<std::vector<uint8_t>>& msgs,
+                                 const std::vector<uint8_t>& context = {}, bool prehashed = false) {
+    size_t n = pk.size();
+    check_sizes(n, sig.size());
+    check_sizes(n, msgs.size());
+    std::vector<uint64_t> offsets(n + 1, 0);
+    std::vector<uint8_t> data;
+    for (size_t i = 0; i < n; i++) {
+      data.insert(data.end(), msgs[i].begin(), msgs[i].end());
+      offsets[i + 1] = data.size();
+    }
+    std::vector<uint8_t> valid(n);
+    check(ecg_ed448_verify_batch(ctx_, n, reinterpret_cast<const uint8_t*>(pk.data()), reinterpret_cast<const uint8_t*>(sig.data()),
+                                 data.empty() ? nullptr : data.data(), offsets.data(), context.empty() ? nullptr : context.data(),
+                                 context.size(), prehashed ? 1 : 0, valid.data()));
+    return std::vector<bool>(valid.begin(), valid.end());
   }
 
   // ---- widening (SURVEY 8(f)): verification, wire format, key agreement ----

@@ -1,5 +1,6 @@
 /* ecgpu.h — C ABI of libecgpu.so: H100-native batched elliptic-curve scalar multiplication
- * (secp256k1 / NIST P-256 on the hot path, every prime-order Weierstrass curve of the reference, and X448 key exchange).
+ * (secp256k1 / NIST P-256 on the hot path, every prime-order Weierstrass curve of the reference, X448 key exchange and
+ * Ed448 signature verification).
  *
  * The reference (RustCrypto/elliptic-curves @ 739304e) has NO FFI boundary; its seams are Rust traits.
  * Each entry point below names the trait method(s) / function(s) it stands in for (paths relative to the
@@ -277,6 +278,30 @@ ecg_status ecg_field_op_batch(ecg_ctx* ctx, ecg_curve curve, int op, size_t n, c
  * on the scalar or on u). */
 ecg_status ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok);
 
+/* ---- Ed448 (RFC 8032): signature verification on the Edwards curve of ed448-goldilocks ---------------------------------
+ * Ed448 verification over a batch: VerifyingKey::verify_raw / verify_ctx / verify_prehashed
+ * (ed448-goldilocks/src/sign/verifying_key.rs:221-312), including VerifyingKey::from_bytes (:187-198).
+ * pk57: n*57 bytes, sig114: n*114 bytes (R || S), message i = msgs[offsets[i] .. offsets[i+1]) (as in
+ * ecg_hash_to_curve_batch; msgs may be NULL when every message is empty), context / context_len: one context for the
+ * whole call (host pointer, <= 255 bytes, else ECG_EINVAL; the reference would silently wrap `ctx.len() as u8`),
+ * prehashed != 0: Ed448ph (phflag = 1), the message bytes are PH(M) as the caller computed it (verify_prehashed:
+ * SHAKE256(M, 64)).
+ * valid[i] = 1 iff the reference accepts: byte 56 of S is 0, 0 < S < ell, A and R decompress (y is reduced mod p, so
+ * y >= p is accepted; the sign of x is bit 7 of byte 56, bits 0-6 of byte 56 are ignored but still hashed) into the
+ * prime-order subgroup, neither is the identity, and [S]B == R + [k]A with k = SHAKE256(dom4 || R || A || M, 114) mod
+ * ell over the bytes as given.  OpenSSL refuses y >= p, bits 0-6 of byte 56 and accepts S = 0 where the equation holds;
+ * here the reference wins.  Invalid encodings are not API errors: valid[i] = 0.
+ * Errors: ECG_EINVAL (null ctx; null pk57 / sig114 / offsets / valid with n > 0; decreasing offsets; msgs NULL with a
+ * non-empty message; context_len > 255, or a NULL context with context_len > 0) and CUDA errors; n = 0 is ECG_OK.
+ * With ECG_FLAG_DEVICE_PTRS pk57, sig114, msgs, offsets and valid are device pointers (records are read bytewise, any
+ * alignment; offsets 8-byte aligned, read back once to check their order); context stays a host pointer.
+ * ECG_FLAG_ZEROIZE scrubs the staged keys, signatures, messages, offsets and verdicts on the device.
+ * ECG_FLAG_CONSTTIME is accepted and changes nothing: verification handles public data only (the reference's
+ * verify_* are not constant time either), so there is no secret for a constant-time path to protect. */
+ecg_status ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114,
+                                  const uint8_t* msgs, const uint64_t* offsets,
+                                  const uint8_t* context, size_t context_len, int prehashed, uint8_t* valid);
+
 /* ---- measurement helpers (not part of the reference-facing surface) ---- */
 
 /* Integer-pipe microbenchmark on device 0 of the ctx: which = 0 IMAD.WIDE.U32.X carry chains (the
@@ -285,7 +310,8 @@ ecg_status ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint
  * of the named kind, or field multiplications for 3/4). */
 ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double* ops_per_s, double* elapsed_ms);
 
-/* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication, the X448 ladder)
+/* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication, the X448 ladder,
+ * the Ed448 verification kernel)
  * with CUDA events on the launching stream; ecg_timing_read returns the accumulated device milliseconds
  * (max over the ctx's devices per call) and the number of calls since ecg_timing_enable. */
 ecg_status ecg_timing_enable(ecg_ctx* ctx, int on);

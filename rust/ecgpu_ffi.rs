@@ -89,6 +89,11 @@ unsafe extern "C" {
     /// X448 (RFC 7748) over a batch: `x448::x448_unchecked` / `EphemeralSecret::diffie_hellman` (x448/src/lib.rs:25-31,
     /// :159-163); `u56` null: u = 5 (`PublicKey::from`); `ok` (may be null): 0 where `x448::x448` returns `None`
     pub fn ecg_x448_batch(ctx: *mut ecg_ctx, n: usize, k56: *const u8, u56: *const u8, out56: *mut u8, ok: *mut u8) -> i32;
+    /// Ed448 verification over a batch: `VerifyingKey::from_bytes` + `verify_raw` / `verify_ctx` / `verify_prehashed`
+    /// (ed448-goldilocks/src/sign/verifying_key.rs:187-312); message i = `msgs[offsets[i]..offsets[i + 1]]`
+    pub fn ecg_ed448_verify_batch(ctx: *mut ecg_ctx, n: usize, pk57: *const u8, sig114: *const u8, msgs: *const u8,
+                                  offsets: *const u64, context: *const u8, context_len: usize, prehashed: i32,
+                                  valid: *mut u8) -> i32;
     pub fn ecg_kernel_launches(ctx: *const ecg_ctx) -> u64;
 }
 
@@ -142,6 +147,32 @@ impl GpuEngine {
         // SAFETY: k, u (when given), out hold n 56-byte records, ok n bytes.
         let rc = unsafe { ecg_x448_batch(self.ctx, n, k.as_ptr().cast(), u_ptr, out.as_mut_ptr().cast(), ok.as_mut_ptr()) };
         self.check(rc).map(|_| (out, ok.into_iter().map(|b| b != 0).collect()))
+    }
+
+    /// Ed448 verification over a batch, for an engine of any curve: `valid[i]` is whether
+    /// `VerifyingKey::from_bytes(pk[i])` followed by `verify_ctx(sig[i], context, msgs[i])` succeeds (`verify_raw`:
+    /// empty context); with `prehashed`, `verify_prehashed` where `msgs[i]` is PH(M) = SHAKE256(M, 64).  The context is
+    /// at most 255 bytes (longer is `ECG_EINVAL`, where the reference would wrap its length byte).
+    pub fn batch_verify_ed448(&mut self, pk: &[[u8; 57]], sig: &[[u8; 114]], msgs: &[&[u8]], context: &[u8],
+                              prehashed: bool) -> Result<Vec<bool>, GpuError> {
+        let n = pk.len();
+        assert!(sig.len() == n && msgs.len() == n);
+        let mut offsets = Vec::with_capacity(n + 1);
+        let mut data = Vec::new();
+        offsets.push(0u64);
+        for m in msgs {
+            data.extend_from_slice(m);
+            offsets.push(data.len() as u64);
+        }
+        let mut valid = vec![0u8; n];
+        let data_ptr = if data.is_empty() { core::ptr::null() } else { data.as_ptr() };
+        let ctx_ptr = if context.is_empty() { core::ptr::null() } else { context.as_ptr() };
+        // SAFETY: pk, sig hold n records of 57 / 114 bytes, offsets n + 1 entries into data, valid n bytes.
+        let rc = unsafe {
+            ecg_ed448_verify_batch(self.ctx, n, pk.as_ptr().cast(), sig.as_ptr().cast(), data_ptr, offsets.as_ptr(), ctx_ptr,
+                                   context.len(), prehashed as i32, valid.as_mut_ptr())
+        };
+        self.check(rc).map(|_| valid.into_iter().map(|b| b != 0).collect())
     }
 
     /// `out[i] = k[i] * P[i]` — batch form of `Mul<Scalar> for ProjectivePoint` / `MulVartime`.

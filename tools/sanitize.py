@@ -75,6 +75,15 @@ def main():
         assert out[i].tobytes() == x448_model.x448(k448[i], u448[i]) and ok[i] == x448_model.u_ok(u448[i]), ("x448", i)
     pub, _ = eng.x448(np.frombuffer(b"".join(k448[:4]), np.uint8))
     assert pub[0].tobytes() == x448_model.x448(k448[0], x448_model.GENERATOR)
+    # Ed448: a few model-made signatures with a context, one empty message, one corrupted signature
+    import ed448_model
+    seed, ctx = os.urandom(57), b"sanitize"
+    pk57 = ed448_model.public_key(seed)
+    m448 = [b"", os.urandom(100), os.urandom(300)]
+    s448 = [ed448_model.sign(seed, m, ctx) for m in m448]
+    s448[2] = s448[2][:60] + bytes([s448[2][60] ^ 1]) + s448[2][61:]
+    v = eng.ed448_verify(np.frombuffer(pk57 * 3, np.uint8), np.frombuffer(b"".join(s448), np.uint8), m448, ctx)
+    assert list(v) == [1, 1, 0], ("ed448", list(v))
     eng.close()
     print("sanitize workload OK")
 
