@@ -17,7 +17,8 @@
 //   ECG_TU 1: sm2, brainpoolP256r1/t1, bign-curve256v1 (8 limbs)   ECG_TU 2: brainpoolP384r1/t1 (12 limbs)
 //   ECG_TU 3: P-224 (7 limbs), P-192 (6 limbs)                    ECG_TU 4: P-521 (17 limbs, 66-byte records)
 //   ECG_TU 5: X448 (Curve448, 14 limbs, 56-byte records): the host pipeline and the ladder kernel, no Weierstrass code
-//   ECG_TU 6: Ed448 verification (the Edwards group on the Curve448 field, SHAKE256): the host pipeline and its kernel
+//   ECG_TU 6: Ed448 (the Edwards group on the Curve448 field): verification (SHAKE256) and the group operations, the
+//             host pipelines and their kernels
 // The groups 1-3 run the generic kernels over the generic Montgomery field policy (ecg_fe_mont.cuh).
 #ifndef ECG_TU
 #define ECG_TU 0
@@ -28,11 +29,12 @@
 #if ECG_TU == 5
 #include "ecg_x448.cuh"
 #else
-#include "ecg_ed448.cuh"
+#include "ecg_ed448_group.cuh"
 #endif
 using namespace ecg;
 // the status flags of ecg_kernels.cuh that finish() reads; every 56-byte string is a valid X448 input, and an Ed448
-// encoding that does not decode is a verdict (valid = 0), so neither kernel reports any
+// encoding that does not decode is a verdict of verification (valid = 0); the Ed448 group kernels report refused scalars
+// and points with the same two bits (ED448G_ERR_SCALAR, ED448G_ERR_POINT)
 #define ERRF_SCALAR 1u
 #define ERRF_POINT 2u
 #define ERRF_SKEW 4u
@@ -87,6 +89,7 @@ struct DevState {
   int dev = 0;
   Lane lane[2];
   uint32_t* fb_table[ECG_CURVE_COUNT] = {nullptr};  // per curve, built lazily (like the reference's LazyLock table)
+  uint32_t* ed448_table = nullptr;                  // the Ed448 fixed-base table, built lazily (ecg_ed448_group.cuh)
   int sm_count = 132;
 };
 
@@ -210,6 +213,7 @@ extern "C" void ecg_ctx_destroy(ecg_ctx* ctx) {
     }
     for (int i = 0; i < ECG_CURVE_COUNT; i++)
       if (d.fb_table[i]) cudaFree(d.fb_table[i]);
+    if (d.ed448_table) cudaFree(d.ed448_table);
   }
   delete ctx;
 }
@@ -2326,6 +2330,289 @@ ECG_API(ecg_ed448_verify_batch)(ecg_ctx* ctx, size_t n, const uint8_t* pk57, con
   if (context_len) memcpy(dom.b + 10, context, context_len);
   dom.len = (uint32_t)(10 + context_len);
   st = ed448_run(ctx, n, pk57, sig114, msgs, offsets, dom, valid);
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+#endif
+
+// ---- Ed448 group operations (ecg_ed448_group.cuh): group 6 holds the kernels; the public symbols (group 0) forward there --
+#if ECG_TU == 0
+__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_mul_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57,
+                                                                              uint8_t* out57);
+__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57);
+__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57,
+                                                                            uint8_t* out57);
+extern "C" ecg_status ecg_ed448_mul_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
+  return ecg_tu6_ecg_ed448_mul_batch(ctx, n, k57, P57, out57);
+}
+extern "C" ecg_status ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57) {
+  return ecg_tu6_ecg_ed448_mul_gen_batch(ctx, n, k57, out57);
+}
+extern "C" ecg_status ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
+  return ecg_tu6_ecg_ed448_lincomb(ctx, n, k57, P57, out57);
+}
+#elif ECG_TU == 6
+static const size_t ED448G_PT = 56 * 4;  // bytes of one extended point
+
+// [k_i] P_i (p57 == nullptr: P_i = B) for cnt elements into ext (SoA, stride cnt); base = index of the first element
+static ecg_status ed448g_launch_mul(ecg_ctx* ctx, Lane& L, const uint8_t* k57, const uint8_t* p57, size_t cnt, size_t base, uint32_t* ext) {
+  const bool scrub = (ctx->flags & ECG_FLAG_ZEROIZE) != 0;
+  if (ctx->flags & ECG_FLAG_CONSTTIME)
+    ed448g_mul_kernel<FpEd448, true><<<grid_for(cnt, ED448G_BLOCK), ED448G_BLOCK, 0, L.s()>>>(k57, p57, cnt, base, ext, L.status, scrub);
+  else
+    ed448g_mul_kernel<FpEd448, false><<<grid_for(cnt, ED448G_BLOCK), ED448G_BLOCK, 0, L.s()>>>(k57, p57, cnt, base, ext, L.status, scrub);
+  LAUNCHED(ctx);
+  return ECG_OK;
+}
+// n extended points (SoA in ext) -> out: compressed 57-byte records, or (TABLE) fixed-base table entries
+template <bool TABLE>
+static ecg_status ed448g_norm(ecg_ctx* ctx, Lane& L, const uint32_t* ext, size_t n, void* out) {
+  ST_TRY(ensure(ctx, L, B_SCR, n * 56));
+  const size_t threads = (n + ED448G_NORM_SLICE - 1) / ED448G_NORM_SLICE;
+  ed448g_norm_kernel<FpEd448, TABLE><<<grid_for(threads, ED448G_BLOCK), ED448G_BLOCK, 0, L.s()>>>(ext, n, (uint32_t*)L.buf[B_SCR], out);
+  LAUNCHED(ctx);
+  return ECG_OK;
+}
+// the fixed-base table of device d, built at its first use: the scalars (2j + 1) 2^(W i) mod ell on the host, their
+// multiples of B by the variable-base kernel, then normalised into (x, y, d x y) entries; freed with the ctx
+static ecg_status ensure_ed448_table(ecg_ctx* ctx, DevState& d) {
+  if (d.ed448_table) return ECG_OK;
+  uint32_t ell[14];
+  CU_TRY(ctx, cudaMemcpyFromSymbol(ell, ED448_L, sizeof ell));
+  const size_t m = (size_t)ED448_FBND * ED448_FBE;
+  std::vector<uint8_t> ks(m * 57, 0);
+  for (int j = 0; j < ED448_FBE; j++) {
+    uint32_t v[14] = {(uint32_t)(2 * j + 1)};
+    for (int i = 0; i < ED448_FBND; i++) {
+      uint8_t* r = &ks[57 * ((size_t)ED448_FBE * i + j)];
+      for (int b = 0; b < 56; b++) r[b] = (uint8_t)(v[b / 4] >> (8 * (b % 4)));
+      for (int s = 0; s < ED448_FBW; s++) {  // v = 2 v mod ell (v < ell < 2^446: no bit leaves the 14 words)
+        uint32_t t[14], c = 0;
+        for (int w = 0; w < 14; w++) {
+          const uint32_t nv = (v[w] << 1) | c;
+          c = v[w] >> 31;
+          v[w] = nv;
+        }
+        uint32_t borrow = 0;
+        for (int w = 0; w < 14; w++) {
+          const uint64_t df = (uint64_t)v[w] - ell[w] - borrow;
+          t[w] = (uint32_t)df;
+          borrow = (uint32_t)(df >> 63);
+        }
+        if (!borrow) memcpy(v, t, sizeof t);
+      }
+    }
+  }
+  Lane& L = d.lane[0];
+  ST_TRY(begin_lane(ctx, L));
+  uint32_t* tab = nullptr;
+  CU_TRY(ctx, cudaMalloc((void**)&tab, (size_t)ED448_FB_WORDS * 4));
+  ecg_status st = ECG_OK;
+  if ((st = ensure(ctx, L, B_A, m * 57)) != ECG_OK || (st = ensure(ctx, L, B_JAC2, m * ED448G_PT)) != ECG_OK) {
+    cudaFree(tab);
+    return st;
+  }
+  uint32_t* ext = (uint32_t*)L.buf[B_JAC2];
+  if (cudaMemcpyAsync(L.buf[B_A], ks.data(), ks.size(), cudaMemcpyHostToDevice, L.s()) == cudaSuccess) {
+    ed448g_mul_kernel<FpEd448, false><<<grid_for(m, ED448G_BLOCK), ED448G_BLOCK, 0, L.s()>>>((const uint8_t*)L.buf[B_A], nullptr, m, 0, ext,
+                                                                                             L.status, false);
+    ctx->launches++;
+    st = ed448g_norm<true>(ctx, L, ext, m, tab);
+  }
+  const cudaError_t e = cudaStreamSynchronize(L.s());
+  if (st != ECG_OK || e != cudaSuccess || cudaGetLastError() != cudaSuccess) {
+    cudaFree(tab);
+    if (st == ECG_OK) ctx->err = "ecg_ed448_mul_gen_batch: building the fixed-base table failed";
+    return st != ECG_OK ? st : ECG_ECUDA;
+  }
+  d.ed448_table = tab;
+  return ECG_OK;
+}
+// one chunk of ecg_ed448_mul_batch (gen = false) or ecg_ed448_mul_gen_batch (gen = true): stage the records, one scalar
+// multiplication per thread, normalise and compress, copy the records back
+static ecg_status ed448g_chunk(ecg_ctx* ctx, DevState& d, Lane& L, bool gen, size_t off, size_t cnt, const uint8_t* k57, const uint8_t* p57,
+                               uint8_t* out57) {
+  DevPtrs dp;
+  ST_TRY(begin_lane(ctx, L));
+  ST_TRY(stage_in(ctx, L, B_K, k57, off, cnt, 57, &dp.k));
+  ST_TRY(stage_in(ctx, L, B_P, gen ? nullptr : p57, off, cnt, 57, &dp.p));
+  ST_TRY(ensure(ctx, L, B_JAC, cnt * ED448G_PT));
+  ST_TRY(stage_out(ctx, L, off, cnt, out57, 57, nullptr, dp));
+  uint32_t* ext = (uint32_t*)L.buf[B_JAC];
+  DOM_BEGIN(ctx, L);
+  if (gen && !(ctx->flags & ECG_FLAG_CONSTTIME)) {
+    ed448g_fixed_kernel<FpEd448><<<grid_for(cnt, ED448G_BLOCK), ED448G_BLOCK, 0, L.s()>>>(dp.k, cnt, off, d.ed448_table, ext, L.status);
+    LAUNCHED(ctx);
+  } else {
+    ST_TRY(ed448g_launch_mul(ctx, L, dp.k, dp.p, cnt, off, ext));  // CONSTTIME k B: the variable-base routine on B
+  }
+  DOM_END(ctx, L);
+  ST_TRY(ed448g_norm<false>(ctx, L, ext, cnt, dp.out));
+  return copy_back(ctx, L, off, cnt, out57, 57, nullptr, dp);
+}
+// the batch split of x448_run: device-pointer mode in DEV_CHUNK pieces on lane 0; host mode sharded over the devices and
+// cut into whole waves of the kernel, alternating lanes so that copies overlap the kernels
+static ecg_status ed448g_run(ecg_ctx* ctx, bool gen, size_t n, const uint8_t* k57, const uint8_t* p57, uint8_t* out57) {
+  const bool table = gen && !(ctx->flags & ECG_FLAG_CONSTTIME);
+  const size_t minblk = table ? ED448G_FB_MINBLK : ED448G_MINBLK;
+  if (ctx->devptr()) {
+    DevState& d = ctx->devs[0];
+    CU_TRY(ctx, cudaSetDevice(d.dev));
+    if (table) ST_TRY(ensure_ed448_table(ctx, d));
+    for (size_t lo = 0; lo < n; lo += DEV_CHUNK) ST_TRY(ed448g_chunk(ctx, d, d.lane[0], gen, lo, std::min(DEV_CHUNK, n - lo), k57, p57, out57));
+    return finish(ctx);
+  }
+  std::vector<Shard> shards = make_shards(n, ctx->devs.size());
+  std::vector<std::vector<Shard>> sched(shards.size());
+  size_t maxchunks = 0;
+  for (size_t i = 0; i < shards.size(); i++) {
+    if (table && shards[i].cnt) {
+      CU_TRY(ctx, cudaSetDevice(ctx->devs[i].dev));
+      ST_TRY(ensure_ed448_table(ctx, ctx->devs[i]));
+    }
+    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * minblk * ED448G_BLOCK);
+    maxchunks = std::max(maxchunks, sched[i].size());
+  }
+  for (size_t c = 0; c < maxchunks; c++) {
+    for (size_t i = 0; i < ctx->devs.size(); i++) {
+      if (c >= sched[i].size()) continue;
+      DevState& d = ctx->devs[i];
+      CU_TRY(ctx, cudaSetDevice(d.dev));
+      ST_TRY(ed448g_chunk(ctx, d, d.lane[c & 1], gen, shards[i].off + sched[i][c].off, sched[i][c].cnt, k57, p57, out57));
+    }
+  }
+  return finish(ctx);
+}
+// the sum of n extended points (SoA in a, stride n), 32 to 1 per pass, ping-ponging through b; the result's word w goes
+// to dst[w * dst_stride]
+static ecg_status ed448g_reduce(ecg_ctx* ctx, Lane& L, uint32_t* a, uint32_t* b, size_t n, uint32_t* dst, size_t dst_stride) {
+  while (n > 32) {
+    const size_t m = (n + 31) / 32;
+    ed448g_sum_kernel<FpEd448><<<grid_for(m, ED448G_BLOCK), ED448G_BLOCK, 0, L.s()>>>(a, n, b, m, m);
+    LAUNCHED(ctx);
+    std::swap(a, b);
+    n = m;
+  }
+  ed448g_sum_kernel<FpEd448><<<1, ED448G_BLOCK, 0, L.s()>>>(a, n, dst, 1, dst_stride);
+  LAUNCHED(ctx);
+  return ECG_OK;
+}
+// sum of [k_i] P_i over [off, off + cnt) on device d (lane 0), in pieces of at most DEV_CHUNK terms: each piece's
+// products are summed into one slot of B_V1, the slots into B_V2 (one extended point, *res)
+static ecg_status ed448g_lincomb_shard(ecg_ctx* ctx, DevState& d, size_t off, size_t cnt, const uint8_t* k57, const uint8_t* p57,
+                                       uint32_t** res) {
+  Lane& L = d.lane[0];
+  ST_TRY(begin_lane(ctx, L));
+  const size_t pieces = (cnt + DEV_CHUNK - 1) / DEV_CHUNK, first = std::min(DEV_CHUNK, cnt);
+  ST_TRY(ensure(ctx, L, B_V1, pieces * ED448G_PT));
+  ST_TRY(ensure(ctx, L, B_V2, ED448G_PT));
+  ST_TRY(ensure(ctx, L, B_JAC, first * ED448G_PT));
+  ST_TRY(ensure(ctx, L, B_JAC2, (first + 31) / 32 * ED448G_PT));
+  uint32_t* part = (uint32_t*)L.buf[B_V1];
+  for (size_t pc = 0; pc < pieces; pc++) {
+    const size_t lo = off + pc * DEV_CHUNK, m = std::min(DEV_CHUNK, off + cnt - lo);
+    DevPtrs dp;
+    ST_TRY(stage_in(ctx, L, B_K, k57, lo, m, 57, &dp.k));
+    ST_TRY(stage_in(ctx, L, B_P, p57, lo, m, 57, &dp.p));
+    DOM_BEGIN(ctx, L);
+    ST_TRY(ed448g_launch_mul(ctx, L, dp.k, dp.p, m, lo, (uint32_t*)L.buf[B_JAC]));
+    DOM_END(ctx, L);
+    ST_TRY(ed448g_reduce(ctx, L, (uint32_t*)L.buf[B_JAC], (uint32_t*)L.buf[B_JAC2], m, part + pc, pieces));
+  }
+  ST_TRY(ed448g_reduce(ctx, L, part, (uint32_t*)L.buf[B_JAC2], pieces, (uint32_t*)L.buf[B_V2], 1));
+  *res = (uint32_t*)L.buf[B_V2];
+  return ECG_OK;
+}
+// one point (56 words at pt) -> the compressed record out57 (a caller pointer), on lane 0 of device d
+static ecg_status ed448g_finish_point(ecg_ctx* ctx, DevState& d, const uint32_t* pt, uint8_t* out57) {
+  Lane& L = d.lane[0];
+  DevPtrs dp;
+  ST_TRY(stage_out(ctx, L, 0, 1, out57, 57, nullptr, dp));
+  ST_TRY(ed448g_norm<false>(ctx, L, pt, 1, dp.out));
+  return copy_back(ctx, L, 0, 1, out57, 57, nullptr, dp);
+}
+// every device's shard is enqueued before any is waited for; the partial sums come back through pinned host memory and
+// device 0 adds them
+static ecg_status ed448g_lincomb_run(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* p57, uint8_t* out57) {
+  const size_t nd = ctx->devs.size();
+  std::vector<Shard> shards = make_shards(n, nd);
+  if (nd == 1) {
+    DevState& d = ctx->devs[0];
+    CU_TRY(ctx, cudaSetDevice(d.dev));
+    uint32_t* res = nullptr;
+    ST_TRY(ed448g_lincomb_shard(ctx, d, 0, n, k57, p57, &res));
+    ST_TRY(ed448g_finish_point(ctx, d, res, out57));
+    return finish(ctx);
+  }
+  for (size_t i = 0; i < nd; i++) {
+    if (shards[i].cnt == 0) continue;
+    DevState& d = ctx->devs[i];
+    CU_TRY(ctx, cudaSetDevice(d.dev));
+    uint32_t* res = nullptr;
+    ST_TRY(ed448g_lincomb_shard(ctx, d, shards[i].off, shards[i].cnt, k57, p57, &res));
+    CU_TRY(ctx, cudaMemcpyAsync(d.lane[0].h_point(), res, ED448G_PT, cudaMemcpyDeviceToHost, d.lane[0].s()));
+  }
+  ST_TRY(finish(ctx));
+  // the partial sums as SoA (stride nd); an empty shard contributes the identity (0 : 1 : 1 : 0)
+  std::vector<uint32_t> parts(56 * nd, 0);
+  for (size_t i = 0; i < nd; i++) {
+    if (shards[i].cnt) {
+      const uint32_t* h = reinterpret_cast<const uint32_t*>(ctx->devs[i].lane[0].h_point());
+      for (int w = 0; w < 56; w++) parts[w * nd + i] = h[w];
+    } else {
+      parts[14 * nd + i] = parts[28 * nd + i] = 1;
+    }
+  }
+  DevState& d = ctx->devs[0];
+  Lane& L = d.lane[0];
+  CU_TRY(ctx, cudaSetDevice(d.dev));
+  ST_TRY(begin_lane(ctx, L));
+  ST_TRY(ensure(ctx, L, B_V3, nd * ED448G_PT));
+  ST_TRY(ensure(ctx, L, B_V4, nd * ED448G_PT));
+  ST_TRY(ensure(ctx, L, B_V2, ED448G_PT));
+  CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_V3], parts.data(), nd * ED448G_PT, cudaMemcpyHostToDevice, L.s()));
+  ST_TRY(ed448g_reduce(ctx, L, (uint32_t*)L.buf[B_V3], (uint32_t*)L.buf[B_V4], nd, (uint32_t*)L.buf[B_V2], 1));
+  ST_TRY(ed448g_finish_point(ctx, d, (const uint32_t*)L.buf[B_V2], out57));
+  return finish(ctx);
+}
+ECG_API(ecg_ed448_mul_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
+  if (!ctx) return ECG_EINVAL;
+  if (n == 0) return ECG_OK;
+  if (!k57 || !P57 || !out57) {
+    ctx->err = "ecg_ed448_mul_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = ed448g_run(ctx, false, n, k57, P57, out57);
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+ECG_API(ecg_ed448_mul_gen_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57) {
+  if (!ctx) return ECG_EINVAL;
+  if (n == 0) return ECG_OK;
+  if (!k57 || !out57) {
+    ctx->err = "ecg_ed448_mul_gen_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = ed448g_run(ctx, true, n, k57, nullptr, out57);
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+ECG_API(ecg_ed448_lincomb)(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
+  if (!ctx) return ECG_EINVAL;
+  if (!out57 || (n > 0 && (!k57 || !P57))) {
+    ctx->err = "ecg_ed448_lincomb: null pointer";
+    return ECG_EINVAL;
+  }
+  if (n == 0) {  // the identity, 01 00 .. 00
+    uint8_t id[57];
+    memset(id, 0, sizeof id);
+    id[0] = 1;
+    if (ctx->devptr()) {
+      CU_TRY(ctx, cudaSetDevice(ctx->devs[0].dev));
+      CU_TRY(ctx, cudaMemcpy(out57, id, 57, cudaMemcpyHostToDevice));
+    } else {
+      memcpy(out57, id, 57);
+    }
+    return ECG_OK;
+  }
+  ecg_status st = ed448g_lincomb_run(ctx, n, k57, P57, out57);
   return st == ECG_OK ? st : fail(ctx, st);
 }
 #endif

@@ -11,6 +11,9 @@ bench.py.  It mirrors the reference's names for the hot path:
     Engine.field_op(curve, op, a, b)           FieldElement add/sub/neg/mul/square/invert
     Engine.x448(k56, u56)                      x448::x448_unchecked / EphemeralSecret::diffie_hellman (x448/src/lib.rs)
     Engine.ed448_verify(pk57, sig114, msgs)    ed448 VerifyingKey::verify_raw / verify_ctx / verify_prehashed
+    Engine.ed448_mul(k57, P57)                 EdwardsPoint * EdwardsScalar over a batch (edwards/extended.rs:698-741)
+    Engine.ed448_mul_gen(k57)                  EdwardsPoint::mul_by_generator over a batch
+    Engine.ed448_lincomb(k57, P57)             LinearCombination::lincomb for EdwardsPoint (extended.rs:310-312)
 
 Buffers are numpy uint8 arrays (host mode) or raw device pointers (device mode, ECG_FLAG_DEVICE_PTRS).
 There is NO CPU fallback: if libecgpu.so is missing, or no CUDA device is present, construction raises.
@@ -55,7 +58,7 @@ EXPORTS = [
     "ecg_schnorr_verify_batch", "ecg_ecdsa_verify_batch", "ecg_decompress_batch",
     "ecg_batch_normalize_hom", "ecg_mul_batch_x", "ecg_field_sqrt_batch",
     "ecg_hash_to_curve_batch", "ecg_hash_to_scalar_batch", "ecg_sm2dsa_verify_batch", "ecg_ecdsa_recover_batch",
-    "ecg_x448_batch", "ecg_ed448_verify_batch",
+    "ecg_x448_batch", "ecg_ed448_verify_batch", "ecg_ed448_mul_batch", "ecg_ed448_mul_gen_batch", "ecg_ed448_lincomb",
 ]
 
 
@@ -145,6 +148,12 @@ def load_library(path: Optional[str] = None) -> ctypes.CDLL:
     lib.ecg_x448_batch.restype = ctypes.c_int
     lib.ecg_ed448_verify_batch.argtypes = [vp, sz, u8p, u8p, u8p, u8p, u8p, sz, ctypes.c_int, u8p]
     lib.ecg_ed448_verify_batch.restype = ctypes.c_int
+    lib.ecg_ed448_mul_batch.argtypes = [vp, sz, u8p, u8p, u8p]
+    lib.ecg_ed448_mul_batch.restype = ctypes.c_int
+    lib.ecg_ed448_mul_gen_batch.argtypes = [vp, sz, u8p, u8p]
+    lib.ecg_ed448_mul_gen_batch.restype = ctypes.c_int
+    lib.ecg_ed448_lincomb.argtypes = [vp, sz, u8p, u8p, u8p]
+    lib.ecg_ed448_lincomb.restype = ctypes.c_int
     lib.ecg_version.argtypes = []
     lib.ecg_version.restype = ctypes.c_char_p
     if path is None:
@@ -553,6 +562,34 @@ class Engine:
                                                     1 if prehashed else 0, _ptr(valid)))
         return valid
 
+    def ed448_mul(self, k57, P57, out=None):
+        """Ed448 group: out[i] = [k[i]] P[i] (n x 57 compressed records; EdwardsPoint * EdwardsScalar).  Scalars are 57-byte
+        little-endian, accepted iff bytes 0..55 < ell (ScalarRangeError with the smallest index otherwise); points are
+        compressed Edwards y, accepted iff CompressedEdwardsY::decompress accepts them (NotOnCurveError otherwise)."""
+        n = np.asarray(k57).size // 57
+        k57 = _u8(k57, 57 * n, "k57")
+        P57 = _u8(P57, 57 * n, "P57")
+        out = _out(out, 57 * n, "out")
+        self._check(self.lib.ecg_ed448_mul_batch(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out)))
+        return out.reshape(n, 57)
+
+    def ed448_mul_gen(self, k57, out=None):
+        """Ed448 group: out[i] = [k[i]] B (EdwardsPoint::mul_by_generator), n x 57 compressed records"""
+        n = np.asarray(k57).size // 57
+        k57 = _u8(k57, 57 * n, "k57")
+        out = _out(out, 57 * n, "out")
+        self._check(self.lib.ecg_ed448_mul_gen_batch(self._ctx, n, _ptr(k57), _ptr(out)))
+        return out.reshape(n, 57)
+
+    def ed448_lincomb(self, k57, P57):
+        """Ed448 group: sum_i [k[i]] P[i] as one 57-byte compressed record (n = 0: the identity 01 00 .. 00)"""
+        n = np.asarray(k57).size // 57
+        k57 = _u8(k57, 57 * n, "k57")
+        P57 = _u8(P57, 57 * n, "P57")
+        out = np.empty(57, np.uint8)
+        self._check(self.lib.ecg_ed448_lincomb(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out)))
+        return out
+
     # ---- raw-pointer API (device_ptrs=True): all arguments are integer CUDA device addresses ----
     def mul_batch_ptr(self, curve, n, k, P_xy, P_inf, out_xy, out_inf):
         self._check(self.lib.ecg_mul_batch(self._ctx, CURVE_IDS[curve], n, _ptr(k), _ptr(P_xy), _ptr(P_inf), _ptr(out_xy), _ptr(out_inf)))
@@ -582,6 +619,18 @@ class Engine:
         ctx = np.frombuffer(bytes(context), np.uint8).copy() if len(context) else None
         self._check(self.lib.ecg_ed448_verify_batch(self._ctx, n, _ptr(pk57), _ptr(sig114), _ptr(msgs), _ptr(offsets), _ptr(ctx), len(context),
                                                     1 if prehashed else 0, _ptr(valid)))
+
+    def ed448_mul_ptr(self, n, k57, P57, out57):
+        """ecg_ed448_mul_batch on device buffers (57-byte records at any alignment)"""
+        self._check(self.lib.ecg_ed448_mul_batch(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out57)))
+
+    def ed448_mul_gen_ptr(self, n, k57, out57):
+        """ecg_ed448_mul_gen_batch on device buffers"""
+        self._check(self.lib.ecg_ed448_mul_gen_batch(self._ctx, n, _ptr(k57), _ptr(out57)))
+
+    def ed448_lincomb_ptr(self, n, k57, P57, out57):
+        """ecg_ed448_lincomb on device buffers (out57: 57 bytes)"""
+        self._check(self.lib.ecg_ed448_lincomb(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out57)))
 
     def timing_enable(self, on: bool = True):
         self._check(self.lib.ecg_timing_enable(self._ctx, 1 if on else 0))

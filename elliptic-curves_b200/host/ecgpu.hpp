@@ -13,6 +13,8 @@
 //                                                         hash2curve::hash_to_scalar (hash2curve/src/group_digest.rs:88-143)
 //   Engine::x448(k, u)                                <->  x448::x448_unchecked / EphemeralSecret::diffie_hellman (x448/src/lib.rs)
 //   Engine::ed448_verify(pk, sig, msgs, ctx, ph)      <->  ed448 VerifyingKey::verify_raw / verify_ctx / verify_prehashed
+//   Engine::ed448_mul / ed448_mul_gen / ed448_lincomb <->  EdwardsPoint * EdwardsScalar, Group::mul_by_generator,
+//                                                         LinearCombination::lincomb (ed448-goldilocks/src/edwards/extended.rs)
 // The typed surface below is for the 256-bit curves with big-endian records (secp256k1, P-256, sm2, brainpoolP256r1/t1);
 // the other curves of include/ecgpu.h (48 / 28 / 24-byte records, bign's little-endian records) are reached through the
 // C ABI directly or the Python mirror, which sizes its buffers per curve.
@@ -170,6 +172,31 @@ class Engine {
                                  data.empty() ? nullptr : data.data(), offsets.data(), context.empty() ? nullptr : context.data(),
                                  context.size(), prehashed ? 1 : 0, valid.data()));
     return std::vector<bool>(valid.begin(), valid.end());
+  }
+
+  // ---- Ed448 group operations, 57-byte scalars and compressed points; the same on an Engine of any curve ----
+  using Ed448Scalar = std::array<uint8_t, 57>;
+  using Ed448Point = std::array<uint8_t, 57>;
+  // out[i] = [k[i]] P[i]: EdwardsPoint * EdwardsScalar (ed448-goldilocks/src/edwards/extended.rs:698-741)
+  std::vector<Ed448Point> ed448_mul(const std::vector<Ed448Scalar>& k, const std::vector<Ed448Point>& P) {
+    check_sizes(k.size(), P.size());
+    std::vector<Ed448Point> out(k.size());
+    check(ecg_ed448_mul_batch(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<const uint8_t*>(P.data()),
+                              reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+  // out[i] = [k[i]] B: Group::mul_by_generator
+  std::vector<Ed448Point> ed448_mul_gen(const std::vector<Ed448Scalar>& k) {
+    std::vector<Ed448Point> out(k.size());
+    check(ecg_ed448_mul_gen_batch(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+  // sum [k[i]] P[i]: LinearCombination::lincomb (empty input: the identity 01 00 .. 00)
+  Ed448Point ed448_lincomb(const std::vector<Ed448Scalar>& k, const std::vector<Ed448Point>& P) {
+    check_sizes(k.size(), P.size());
+    Ed448Point out{};
+    check(ecg_ed448_lincomb(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<const uint8_t*>(P.data()), out.data()));
+    return out;
   }
 
   // ---- widening (SURVEY 8(f)): verification, wire format, key agreement ----

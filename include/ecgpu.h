@@ -1,6 +1,6 @@
 /* ecgpu.h — C ABI of libecgpu.so: H100-native batched elliptic-curve scalar multiplication
- * (secp256k1 / NIST P-256 on the hot path, every prime-order Weierstrass curve of the reference, X448 key exchange and
- * Ed448 signature verification).
+ * (secp256k1 / NIST P-256 on the hot path, every prime-order Weierstrass curve of the reference, X448 key exchange, and
+ * Ed448 signature verification and group operations).
  *
  * The reference (RustCrypto/elliptic-curves @ 739304e) has NO FFI boundary; its seams are Rust traits.
  * Each entry point below names the trait method(s) / function(s) it stands in for (paths relative to the
@@ -100,7 +100,12 @@ typedef enum {
                                    always takes the per-term path (the bucket method's access pattern is the scalars).
                                    Left data-dependent: the exceptional-case branches of the Jacobian formulas, reachable
                                    only for k = 0 (not a NonZeroScalar) and a negligible set of scalars; kernel timing also
-                                   depends on inputs being rejected.  The default (flag clear) is the vartime analogue. */
+                                   depends on inputs being rejected.  The default (flag clear) is the vartime analogue.
+                                   The Ed448 group entries (ecg_ed448_mul_batch, ecg_ed448_mul_gen_batch,
+                                   ecg_ed448_lincomb) follow the same rule: a masked scan of the 8-entry table, a masked
+                                   negation and a masked "add ell when k is even", k*B through the variable-base routine on
+                                   B.  The Edwards formulas are complete, so that path has no scalar-dependent branch at
+                                   all. */
 
 /* Create a context on the given CUDA devices (NULL/0 = device 0).  With several devices a host-pointer
  * batch is split into contiguous index ranges, one per device (SURVEY.md §8(e)); there is no
@@ -302,6 +307,37 @@ ecg_status ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, c
                                   const uint8_t* msgs, const uint64_t* offsets,
                                   const uint8_t* context, size_t context_len, int prehashed, uint8_t* valid);
 
+/* ---- Ed448 group operations on the Edwards curve of ed448-goldilocks (EdwardsPoint) -------------------------------------
+ * Records: a scalar is 57 bytes little-endian (EdwardsScalarBytes), accepted iff EdwardsScalar::from_repr accepts it
+ * (from_canonical_bytes, ed448-goldilocks/src/edwards/scalar.rs:32-42): bytes 0..55 read as an integer must be < ell,
+ * byte 56 is ignored (its test is ORed with "byte 55 < 64", which every value < ell meets), else ECG_ESCALAR_RANGE.
+ * A point is 57 bytes, accepted iff GroupEncoding::from_bytes / CompressedEdwardsY::decompress accepts it
+ * (edwards/affine.rs:487-520): y = bytes 0..55 little-endian reduced mod p (y >= p is accepted), the sign of x is bit 7 of
+ * byte 56 (bits 0-6 ignored), on the curve and torsion free; the identity 01 00 .. 00 is accepted under either sign bit,
+ * (0, -1) and the all-zero record (a point of order 4) are refused, else ECG_ENOT_ON_CURVE.  An output is
+ * AffinePoint::compress (edwards/affine.rs:29-41): canonical y, byte 56 = (x mod 2) << 7; the identity is 01 00 .. 00.
+ * A refused record fails the whole call; ecg_last_error_index gives the smallest offending index.
+ * The reference's scalar_mul goes through the 4-isogeny ([4 (s / 4 mod ell)]P, edwards/extended.rs:357-365), which is
+ * [s]P on the torsion-free points the encoding admits: the results are the reference's bits.
+ * Errors: ECG_EINVAL (null ctx; a null array with n > 0; for lincomb a null out57 at any n) and CUDA errors.
+ * With ECG_FLAG_DEVICE_PTRS every array is a device pointer, read and written bytewise at any alignment.
+ * ECG_FLAG_ZEROIZE scrubs the staged scalars and points, the per-thread tables, the intermediate points and the
+ * normalisation scratch on the device.  ECG_FLAG_CONSTTIME: see its definition; outputs are identical either way.
+ * A multi-device ctx splits the batch into contiguous index ranges. */
+
+/* out57[i] = [k57[i]] P57[i]: Mul<&EdwardsScalar> / MulVartime for EdwardsPoint (ed448-goldilocks/src/edwards/
+ * extended.rs:698-741) over a batch; n = 0 is ECG_OK. */
+ecg_status ecg_ed448_mul_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57);
+
+/* out57[i] = [k57[i]] B: Group::mul_by_generator for EdwardsPoint (EdwardsPoint::GENERATOR * k; with a clamped
+ * SHAKE256(seed) scalar this is the RFC 8032 public key) over a batch, from a window table built on each device at its
+ * first use (1.2 MB, freed with the ctx); n = 0 is ECG_OK. */
+ecg_status ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57);
+
+/* out57 = sum_i [k57[i]] P57[i]: LinearCombination::lincomb for EdwardsPoint (ed448-goldilocks/src/edwards/
+ * extended.rs:310-312, the reference's default sum of products), one 57-byte record; n = 0 writes the identity. */
+ecg_status ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t out57[57]);
+
 /* ---- measurement helpers (not part of the reference-facing surface) ---- */
 
 /* Integer-pipe microbenchmark on device 0 of the ctx: which = 0 IMAD.WIDE.U32.X carry chains (the
@@ -311,7 +347,7 @@ ecg_status ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, c
 ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double* ops_per_s, double* elapsed_ms);
 
 /* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication, the X448 ladder,
- * the Ed448 verification kernel)
+ * the Ed448 verification kernel, the Ed448 scalar-multiplication kernels)
  * with CUDA events on the launching stream; ecg_timing_read returns the accumulated device milliseconds
  * (max over the ctx's devices per call) and the number of calls since ecg_timing_enable. */
 ecg_status ecg_timing_enable(ecg_ctx* ctx, int on);

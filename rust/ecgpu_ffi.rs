@@ -94,6 +94,13 @@ unsafe extern "C" {
     pub fn ecg_ed448_verify_batch(ctx: *mut ecg_ctx, n: usize, pk57: *const u8, sig114: *const u8, msgs: *const u8,
                                   offsets: *const u64, context: *const u8, context_len: usize, prehashed: i32,
                                   valid: *mut u8) -> i32;
+    /// Ed448 group: `out57[i] = k57[i] * P57[i]` (`Mul<&EdwardsScalar> for EdwardsPoint`, ed448-goldilocks/src/edwards/
+    /// extended.rs:698-741); 57-byte scalars (bytes 0..55 < ell) and compressed points
+    pub fn ecg_ed448_mul_batch(ctx: *mut ecg_ctx, n: usize, k57: *const u8, p57: *const u8, out57: *mut u8) -> i32;
+    /// Ed448 group: `out57[i] = EdwardsPoint::mul_by_generator(k57[i])`
+    pub fn ecg_ed448_mul_gen_batch(ctx: *mut ecg_ctx, n: usize, k57: *const u8, out57: *mut u8) -> i32;
+    /// Ed448 group: `out57 = EdwardsPoint::lincomb(&[(P57[i], k57[i])])` (extended.rs:310-312); n = 0: the identity
+    pub fn ecg_ed448_lincomb(ctx: *mut ecg_ctx, n: usize, k57: *const u8, p57: *const u8, out57: *mut u8) -> i32;
     pub fn ecg_kernel_launches(ctx: *const ecg_ctx) -> u64;
 }
 
@@ -173,6 +180,33 @@ impl GpuEngine {
                                    context.len(), prehashed as i32, valid.as_mut_ptr())
         };
         self.check(rc).map(|_| valid.into_iter().map(|b| b != 0).collect())
+    }
+
+    /// Ed448 group, for an engine of any curve: `out[i] = k[i] * P[i]` (`EdwardsPoint * EdwardsScalar`); a scalar whose
+    /// bytes 0..55 are >= ell or a point `CompressedEdwardsY::decompress` refuses fails the call with its smallest index.
+    pub fn batch_mul_ed448(&mut self, k: &[[u8; 57]], p: &[[u8; 57]]) -> Result<Vec<[u8; 57]>, GpuError> {
+        assert_eq!(k.len(), p.len());
+        let mut out = vec![[0u8; 57]; k.len()];
+        // SAFETY: k, p and out hold k.len() records of 57 bytes.
+        let rc = unsafe { ecg_ed448_mul_batch(self.ctx, k.len(), k.as_ptr().cast(), p.as_ptr().cast(), out.as_mut_ptr().cast()) };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Ed448 group: `out[i] = EdwardsPoint::mul_by_generator(k[i])`
+    pub fn batch_mul_gen_ed448(&mut self, k: &[[u8; 57]]) -> Result<Vec<[u8; 57]>, GpuError> {
+        let mut out = vec![[0u8; 57]; k.len()];
+        // SAFETY: k and out hold k.len() records of 57 bytes.
+        let rc = unsafe { ecg_ed448_mul_gen_batch(self.ctx, k.len(), k.as_ptr().cast(), out.as_mut_ptr().cast()) };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Ed448 group: `sum k[i] * P[i]` (`LinearCombination::lincomb`); empty input gives the identity
+    pub fn lincomb_ed448(&mut self, k: &[[u8; 57]], p: &[[u8; 57]]) -> Result<[u8; 57], GpuError> {
+        assert_eq!(k.len(), p.len());
+        let mut out = [0u8; 57];
+        // SAFETY: k and p hold k.len() records of 57 bytes, out 57 bytes.
+        let rc = unsafe { ecg_ed448_lincomb(self.ctx, k.len(), k.as_ptr().cast(), p.as_ptr().cast(), out.as_mut_ptr()) };
+        self.check(rc).map(|_| out)
     }
 
     /// `out[i] = k[i] * P[i]` — batch form of `Mul<Scalar> for ProjectivePoint` / `MulVartime`.

@@ -84,6 +84,17 @@ def main():
     s448[2] = s448[2][:60] + bytes([s448[2][60] ^ 1]) + s448[2][61:]
     v = eng.ed448_verify(np.frombuffer(pk57 * 3, np.uint8), np.frombuffer(b"".join(s448), np.uint8), m448, ctx)
     assert list(v) == [1, 1, 0], ("ed448", list(v))
+    # Ed448 group operations: one small call per entry, against the model
+    import ed448_group_model
+    kg = [rng.randrange(ed448_model.L) for _ in range(5)]
+    K448 = np.frombuffer(b"".join(ed448_group_model.enc_scalar(k) for k in kg), np.uint8)
+    P448 = np.frombuffer(pk57 * 5, np.uint8)
+    g = eng.ed448_mul_gen(K448)
+    assert [bytes(r) for r in g] == [ed448_group_model.mul_gen(ed448_group_model.enc_scalar(k)) for k in kg], "ed448 mul_gen"
+    m = eng.ed448_mul(K448, P448)
+    assert bytes(m[0]) == ed448_group_model.mul(ed448_group_model.enc_scalar(kg[0]), pk57), "ed448 mul"
+    lc = eng.ed448_lincomb(K448, P448)
+    assert bytes(lc) == ed448_group_model.lincomb([ed448_group_model.enc_scalar(k) for k in kg], [pk57] * 5), "ed448 lincomb"
     eng.close()
     print("sanitize workload OK")
 
