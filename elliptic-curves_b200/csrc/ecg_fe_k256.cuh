@@ -42,7 +42,14 @@ struct FpK256T {
   static constexpr bool DBL_CALL = (OPT & 2048) != 0;
   static constexpr bool MADD_CALL = (OPT & 4096) != 0;
   static constexpr bool DBL_3M5S = false;
-  typedef FpK256T<(OPT & (1 | 8 | 64 | 128))> Inline;  // the same field with mul / sqr inlined
+  // OPT bit 13: the window table of k256_mul_thread carries beta*x beside x, so the lambda-half additions read it
+  // instead of multiplying in the loop (8 M per table instead of 34 M per scalar)
+  static constexpr bool BETA_COLUMN = (OPT & 8192) != 0;
+  // OPT bit 14: the a = 0 doubling forms 3/2 X^2 as X^2 + X^2/2 (carry chains) instead of mul_small(3) then half
+  static constexpr bool HALF3_ADD = (OPT & 16384) != 0;
+  // OPT bit 15: Y3 of the doubling and of the mixed addition is one mul_sub / mul_sub_sqr (two products, one reduction)
+  static constexpr bool MUL_SUB = (OPT & 32768) != 0;
+  typedef FpK256T<(OPT & (1 | 8 | 64 | 128 | 8192 | 16384 | 32768))> Inline;  // the same field with mul / sqr inlined
 
   ECG_D static void set_zero(Fe& r) {
 #pragma unroll
@@ -53,29 +60,35 @@ struct FpK256T {
     r.v[0] = 1;
   }
 
-  // r (8 limbs, already holding the low part) += top * C where top = t0 + 2^32*t1, t1 in {0,1};
-  // the result is again < 2^256 (at most two wrap-arounds, the second confined to limbs 0..1).
-  ECG_D static void fold_top(uint32_t* r, uint32_t t0, uint32_t t1) {
+  // r (8 limbs, already holding the low part) += top * C + e * C^2 where top = t0 + 2^32*t1 <= C, t1 and e in {0,1}
+  // (e is bit 512 of a mul_sub intermediate: 2^512 == C^2 = 2^64 + 1954*2^32 + 954529 (mod p); every other caller
+  // passes e = 0, which folds away at compile time).  The addend is < 2C^2 < 2^67, so the result is again < 2^256
+  // (at most two wrap-arounds, the second confined to limbs 0..3).
+  ECG_D static void fold_top(uint32_t* r, uint32_t t0, uint32_t t1, uint32_t e = 0) {
     uint32_t q0, q1;
     mul_wide(q0, q1, t0, C0);                     // t0*977
-    uint64_t s1 = (uint64_t)q1 + t0 + (t1 ? C0 : 0u);  // position-1 column: hi(t0*977) + t0 + t1*977
+    uint64_t s0 = (uint64_t)q0 + (e ? 954529u : 0u);  // position-0 column: lo(t0*977) + e*lo(C^2)
+    // position-1 column: hi(t0*977) + t0 + t1*977 + e*1954 + carry
+    uint64_t s1 = (uint64_t)q1 + t0 + (t1 ? C0 : 0u) + (e ? 1954u : 0u) + (s0 >> 32);
+    uint32_t q0s = (uint32_t)s0;
     uint32_t p1 = (uint32_t)s1;
-    uint32_t p2 = (uint32_t)(s1 >> 32) + t1;       // position-2 column
-    r[0] = add_cc(r[0], q0);
+    uint32_t p2 = (uint32_t)(s1 >> 32) + t1 + e;  // position-2 column
+    r[0] = add_cc(r[0], q0s);
     r[1] = addc_cc(r[1], p1);
     r[2] = addc_cc(r[2], p2);
 #pragma unroll
     for (int i = 3; i < 8; i++) r[i] = addc_cc(r[i], 0);
     uint32_t cf = addc(0, 0);
-    // wrapped past 2^256 (rare): the residue is < 2^66, add C once more; cannot wrap again.
+    // wrapped past 2^256 (rare): the residue is < 2^67, add C once more; cannot wrap again.
     r[0] = add_cc(r[0], cf ? C0 : 0u);
     r[1] = addc_cc(r[1], cf);
     r[2] = addc_cc(r[2], 0);
     r[3] = addc(r[3], 0);
   }
 
-  // 16-limb t -> r = t mod p (weakly reduced).  t_lo + t_hi * C with the even/odd pair trick, then fold.
-  ECG_D static void reduce16(Fe& r, const uint32_t* t) {
+  // 16-limb t (+ e * 2^512, e in {0,1}) -> r = t mod p (weakly reduced).  t_lo + t_hi * C with the even/odd pair
+  // trick (any t < 2^512: the sum is < 2^256 (1 + C), so its top is <= C), then fold.
+  ECG_D static void reduce16(Fe& r, const uint32_t* t, uint32_t e = 0) {
     uint32_t lo[8], q[8];
 #pragma unroll
     for (int i = 0; i < 8; i++) {
@@ -101,7 +114,45 @@ struct FpK256T {
     for (int k = 2; k < 8; k++) r.v[k] = addc_cc(lo[k], q[k - 1]);
     uint32_t t0 = addc_cc(e8, q[7]);
     uint32_t t1 = addc(q8, 0);  // top = t0 + 2^32*t1 <= C
-    fold_top(r.v, t0, t1);
+    fold_top(r.v, t0, t1, e);
+  }
+  // t (16 limbs) = a*b, u (16 limbs) = c*d, each <= (2^256 - 1)^2 (any operands < 2^256, not only < p)
+  //   -> r = (a*b - c*d) mod p, weakly reduced, with one reduction.  t - u lies in (-2^512, 2^512); when it is negative,
+  // 2p * 2^256 = 2^513 - 2C * 2^256 (== 0 mod p) is added, giving D in (2^512 - 2C * 2^256, 2^513): D = t' + e * 2^512
+  // with t' < 2^512 and e in {0,1}, and reduce16 folds the two together.  t is overwritten.
+  ECG_D static void sub_reduce16(Fe& r, uint32_t* t, const uint32_t* u) {
+    const uint32_t bw = subN<16>(t, t, u);  // t = a*b - c*d + bw * 2^512
+    const uint32_t m = 0u - bw;
+    t[8] = sub_cc(t[8], m & 1954u);  // high half -= bw * 2C  (2C = 2^33 + 1954)
+    t[9] = subc_cc(t[9], m & 2u);
+#pragma unroll
+    for (int i = 10; i < 16; i++) t[i] = subc_cc(t[i], 0);
+    const uint32_t b2 = 0u - subc(0, 0);  // the 2^512 of the correction was consumed (b2 <= bw: D >= 0)
+    reduce16(r, t, bw ^ b2);
+  }
+  ECG_D static void mul_sub(Fe& r, const Fe& a, const Fe& b, const Fe& c, const Fe& d) {
+    uint32_t t[16], u[16];
+    if (OPT & 8) {
+      mul8x8_kara(u, c.v, d.v);
+      mul8x8_kara(t, a.v, b.v);
+    } else {
+      mul8x8(u, c.v, d.v);
+      mul8x8(t, a.v, b.v);
+    }
+    sub_reduce16(r, t, u);
+  }
+  // r = (a*b - c^2) mod p, the same way
+  ECG_D static void mul_sub_sqr(Fe& r, const Fe& a, const Fe& b, const Fe& c) {
+    uint32_t t[16], u[16];
+    if (OPT & 1)
+      sqr8(u, c.v);
+    else
+      mul8x8(u, c.v, c.v);
+    if (OPT & 8)
+      mul8x8_kara(t, a.v, b.v);
+    else
+      mul8x8(t, a.v, b.v);
+    sub_reduce16(r, t, u);
   }
 
   ECG_D static void mul_body(Fe& r, const Fe& a, const Fe& b) {
@@ -291,5 +342,8 @@ struct FpK256T {
 };
 
 typedef FpK256T<ECG_K256_OPT> FpK256;
+// the policy of k256_varbase_kernel: every field operation inlined, and work moved off the multiplier (OPT bits 13-15):
+// beta*x in the window table, 3/2 X^2 by carry chains, Y3 of both point operations with one reduction
+typedef FpK256T<1 | 8192 | 16384 | 32768> FpK256Inline;
 
 }  // namespace ecg

@@ -38,6 +38,7 @@ struct FpP256T {
   // the P-256 squaring is bound by its reduction's adds, not by products: no multiplication-for-squaring trades
   static constexpr bool SQR_TRADE_DBL = false;
   static constexpr bool SQR_TRADE_MADD = false;
+  static constexpr bool HALF3_ADD = false, MUL_SUB = false;  // secp256k1-only doubling / Y3 forms (ecg_fe_k256.cuh)
   static constexpr bool DBL_CALL = (OPT & 2048) != 0;   // see ecg_fe_k256.cuh
   static constexpr bool MADD_CALL = (OPT & 4096) != 0;
   static constexpr bool DBL_3M5S = (OPT & 1024) != 0;   // a = -3 doubling as 3M+5S (Z3 = ((Y+Z)^2 - Y^2 - Z^2)/2) instead of 4M+4S

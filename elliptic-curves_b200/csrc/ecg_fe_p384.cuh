@@ -36,6 +36,7 @@ struct FpP384T {
   static constexpr bool MONT = false;
   static constexpr bool SQR_TRADE_DBL = false;
   static constexpr bool SQR_TRADE_MADD = false;
+  static constexpr bool HALF3_ADD = false, MUL_SUB = false;  // secp256k1-only doubling / Y3 forms (ecg_fe_k256.cuh)
   static constexpr bool DBL_CALL = false;
   static constexpr bool MADD_CALL = false;
   static constexpr bool DBL_3M5S = false;

@@ -80,23 +80,25 @@ ECG_DEV uint32_t load_pair(uint32_t* k, typename C::F::AffT& P, bool& inf, const
 
 // ------------------------------------------------------------------------------------------------
 // Per-thread window tables live in global memory, one slot per block: word w of entry e of thread t at
-// gtab[blockIdx*BLOCK*EW + (e*WPE + w)*BLOCK + t]  (EW = words per thread: 128 affine / 192 Jacobian).
+// gtab[blockIdx*BLOCK*EW + (e*WPE + w)*BLOCK + t]  (EW = words per thread: 192 for 8 secp256k1 entries of (x, y, beta*x)
+// and for 8 Jacobian P-256 entries).
 // A warp's access to one (e, w) of differing e per lane touches 32 distinct 4-byte words spread over at most 8
-// rows; the blocks resident at any time on the 132 SMs of an H100 keep 35 MB (secp256k1) to 65 MB (P-256) of tables live
+// rows; the blocks resident at any time on the 132 SMs of an H100 keep 52 MB (secp256k1) to 65 MB (P-256) of tables live
 // against its 50 MB L2 (a pair reads ~7 KB of table, so what spills costs little HBM bandwidth).  Shared memory
 // was the first home of these tables (512-768 B/thread capped occupancy at 8-12 warps/SM); moving them out lets
 // registers set the occupancy (16-20 warps/SM); tools/kbench.cu times both homes.
-#define K_TAB_WORDS 128  /* 8 affine entries  x 16 words */
+// secp256k1 slots: 8 affine entries x 24 words (x, y, beta*x) for k256_varbase_kernel; the constant-time and a*G + b*P
+// kernels keep 16-word entries (x, y) in the first 128 words of a slot of the same size.
+#define K_TAB_WORDS 192
 #define P_TAB_WORDS 192  /* 8 Jacobian entries x 24 words */
 
 // secp256k1 variable-base: one pair per thread.
-// Field operations fully inlined (FpK256T<1>: no call marshalling) with a block-wide barrier between the doubling phase
+// Field operations fully inlined (FpK256Inline, ecg_fe_k256.cuh: no call marshalling) with a block-wide barrier between the doubling phase
 // and the addition phase of every window (k256_mul_thread<.., 1>): all warps of a block then run the same stretch of
 // code, so only one phase's instructions have to be resident in the instruction cache at a time — the fully inlined
 // body without the barriers thrashes it, the call-based body pays ~21 IMAD.MOV per call on the FMA pipe
 // (tools/kbench.cu times the three forms).
 // Every thread of a block must reach the barriers: out-of-range threads redo the block's last valid pair and store nothing.
-typedef FpK256T<1> FpK256Inline;
 template <int BLOCK, int MINBLK>
 ECG_KERNEL(BLOCK, MINBLK)
     k256_varbase_kernel(const uint8_t* __restrict__ kb, const uint8_t* __restrict__ pxy,
@@ -110,7 +112,7 @@ ECG_KERNEL(BLOCK, MINBLK)
   bool inf;
   uint32_t err = load_pair<CurveK256>(k, P, inf, kb, pxy, pinf, cidx);
   if (err && live) report_error(status, err, base + idx);
-  TabRef tab{gtab + (size_t)blockIdx.x * BLOCK * K_TAB_WORDS + threadIdx.x, (uint32_t)BLOCK};
+  K256TabRef<FpK256Inline> tab{gtab + (size_t)blockIdx.x * BLOCK * K_TAB_WORDS + threadIdx.x, (uint32_t)BLOCK};
   Jac r;
   k256_mul_thread<FpK256Inline, 1>(r, k, P, tab);
   if (!live) return;

@@ -16,30 +16,37 @@
 
 namespace ecg {
 
-// Window-table accessor: entry e (0..7), word w (0..15: x[0..7], y[0..7]) lives at base[(e*16+w)*stride].
+// Window-table accessor: entry e (0..7), word w (0..WPE-1: x[0..NL-1], y[0..NL-1], then with WPE = 3 NL a second
+// x column, beta*x for secp256k1) lives at base[(e*WPE+w)*stride].
 // In the kernels base = slot + threadIdx.x and stride = blockDim.x: the 32 lanes of a warp touch 32 consecutive
 // words of each row they select (coalesced when lanes agree on the entry, at worst 8 rows when they do not).
-template <int NL>
+template <int NL, int WPE = 2 * NL>
 struct TabRefN {
   uint32_t* base;
   uint32_t stride;
   ECG_D void store(int e, const FeN<NL>& x, const FeN<NL>& y) const {
 #pragma unroll
     for (int w = 0; w < NL; w++) {
-      base[(e * 2 * NL + w) * stride] = x.v[w];
-      base[(e * 2 * NL + NL + w) * stride] = y.v[w];
+      base[(e * WPE + w) * stride] = x.v[w];
+      base[(e * WPE + NL + w) * stride] = y.v[w];
     }
   }
-  ECG_D void load(int e, FeN<NL>& x, FeN<NL>& y) const {
+  ECG_D void store_x2(int e, const FeN<NL>& x2) const {  // the second x column (WPE = 3 NL)
+#pragma unroll
+    for (int w = 0; w < NL; w++) base[(e * WPE + 2 * NL + w) * stride] = x2.v[w];
+  }
+  // x from the column starting at word xcol (0, or 2 NL for the second x column), y
+  ECG_D void load(int e, FeN<NL>& x, FeN<NL>& y, int xcol = 0) const {
 #pragma unroll
     for (int w = 0; w < NL; w++) {
-      x.v[w] = base[(e * 2 * NL + w) * stride];
-      y.v[w] = base[(e * 2 * NL + NL + w) * stride];
+      x.v[w] = base[(e * WPE + xcol + w) * stride];
+      y.v[w] = base[(e * WPE + NL + w) * stride];
     }
   }
   // entry `idx` without a secret-dependent address: every entry is read, the wanted one kept by mask
   // (LookupTable::select, primeorder/src/tables/lookup.rs:43-65)
   ECG_D void load_ct(uint32_t idx, FeN<NL>& x, FeN<NL>& y) const {
+    static_assert(WPE == 2 * NL, "the masked scan covers the (x, y) layout only");
 #pragma unroll
     for (int w = 0; w < NL; w++) x.v[w] = y.v[w] = 0;
 #pragma unroll 1
@@ -47,13 +54,16 @@ struct TabRefN {
       const uint32_t m = 0u - (uint32_t)(e == idx);
 #pragma unroll
       for (int w = 0; w < NL; w++) {
-        x.v[w] |= base[(e * 2 * NL + w) * stride] & m;
-        y.v[w] |= base[(e * 2 * NL + NL + w) * stride] & m;
+        x.v[w] |= base[(e * WPE + w) * stride] & m;
+        y.v[w] |= base[(e * WPE + NL + w) * stride] & m;
       }
     }
   }
 };
 typedef TabRefN<8> TabRef;
+// the secp256k1 table of a field policy: (x, y), or (x, y, beta*x) with F::BETA_COLUMN
+template <class F>
+using K256TabRef = TabRefN<8, F::BETA_COLUMN ? 24 : 16>;
 // Same, for Jacobian entries (3*NL words: X, Y, Z).
 template <int NL>
 struct TabRefJN {
@@ -103,9 +113,10 @@ ECG_D void k256_beta(Fe& b) {
 // under (x,y) -> (x Zg^2, y Zg^3): the 8 entries share the denominator Zg, which is returned and
 // multiplied back into the accumulator's Z once at the end.  Valid for a = 0 only (the a=0 doubling and
 // the additions never use the curve constant b, and b is the only coefficient the isomorphism changes).
-// Cost: 1 dbl + 7 madd + 35M rescale, no inversion, no block-level synchronisation.
+// Cost: 1 dbl + 7 madd + 35M rescale, no inversion, no block-level synchronisation.  With F::BETA_COLUMN each entry
+// also gets beta*x (8M more), the x of the endomorphism image (beta x, y) that the lambda half of the scalar adds.
 template <class F>
-ECG_D void build_table_iso_a0(const TabRef& tab, Fe& Zg, const Aff& P) {
+ECG_D void build_table_iso_a0(const K256TabRef<F>& tab, Fe& Zg, const Aff& P) {
   Jac d, cur;
   aff_dbl<F, false>(d, P);  // 2P = (dX, dY, dZ)
   // On E'' = image under dZ: 2P is affine (dX, dY); P becomes (x dZ^2, y dZ^3).
@@ -127,7 +138,12 @@ ECG_D void build_table_iso_a0(const TabRef& tab, Fe& Zg, const Aff& P) {
   }
   // bring entries 0..6 to the denominator of entry 7: scale by zs = Z7/Zi = prod_{j>i} zr[j]
   F::mul(Zg, cur.Z, d.Z);
-  Fe zs = zr[7];
+  Fe zs = zr[7], beta;
+  if constexpr (F::BETA_COLUMN) {
+    k256_beta(beta);
+    F::mul(cur.X, cur.X, beta);
+    tab.store_x2(7, cur.X);
+  }
 #pragma unroll 1
   for (int i = 6; i >= 0; i--) {
     Fe x, y, zz;
@@ -137,6 +153,10 @@ ECG_D void build_table_iso_a0(const TabRef& tab, Fe& Zg, const Aff& P) {
     F::mul(zz, zz, zs);
     F::mul(y, y, zz);
     tab.store(i, x, y);
+    if constexpr (F::BETA_COLUMN) {
+      F::mul(x, x, beta);
+      tab.store_x2(i, x);
+    }
     if (i > 0) F::mul(zs, zs, zr[i]);
   }
 }
@@ -156,12 +176,14 @@ ECG_D void build_table_iso_a0(const TabRef& tab, Fe& Zg, const Aff& P) {
 // of the GLV halves is branch-free, so neither addresses nor branches depend on the scalar (what is left: the
 // exceptional-case branches of the Jacobian formulas, reachable only for k = 0 and a negligible set of scalars).
 template <class F = FpK256, int PHASE_SYNC = 0, bool CT = false>  // PHASE_SYNC: 0 none, 1 per phase (doublings | additions), 2 before every point operation
-ECG_D void k256_mul_thread(Jac& r, const uint32_t* k, const Aff& P, const TabRef& tab) {
+ECG_D void k256_mul_thread(Jac& r, const uint32_t* k, const Aff& P, const K256TabRef<F>& tab) {
   GlvHalf g1, g2;
   glv_split_k256<CT>(g1, g2, k);
   Fe Zg, beta;
   build_table_iso_a0<F>(tab, Zg, P);
   k256_beta(beta);
+  // the lambda half adds (beta x, y): x from the table's beta*x column (word 16 of an entry), or times beta here
+  constexpr int BX = F::BETA_COLUMN ? 16 : 0;
 
   Jac acc;
   Aff e;
@@ -169,8 +191,8 @@ ECG_D void k256_mul_thread(Jac& r, const uint32_t* k, const Aff& P, const TabRef
   tab.load(0, acc.X, acc.Y);
   fe_cneg<F>(acc.Y, g1.neg);
   F::set_one(acc.Z);
-  tab.load(0, e.x, e.y);
-  F::mul(e.x, e.x, beta);
+  tab.load(0, e.x, e.y, BX);
+  if (!F::BETA_COLUMN) F::mul(e.x, e.x, beta);
   fe_cneg<F>(e.y, g2.neg);
   jac_madd<F, false>(acc, acc, e);
 
@@ -190,11 +212,16 @@ ECG_D void k256_mul_thread(Jac& r, const uint32_t* k, const Aff& P, const TabRef
       uint32_t sneg = half ? g2.neg : g1.neg;
       uint32_t pos = n >> 3;                       // digit sign: n>=8 -> positive
       uint32_t idx = pos ? (n & 7u) : (7u - n);
-      if (CT)
-        tab.load_ct(idx, e.x, e.y);
-      else
-        tab.load((int)idx, e.x, e.y);
-      if (half) F::mul(e.x, e.x, beta);
+      if constexpr (F::BETA_COLUMN) {  // x column chosen by address: no product, no branch
+        static_assert(!CT, "the masked scan reads the (x, y) layout");
+        tab.load((int)idx, e.x, e.y, half ? BX : 0);
+      } else {
+        if (CT)
+          tab.load_ct(idx, e.x, e.y);
+        else
+          tab.load((int)idx, e.x, e.y);
+        if (half) F::mul(e.x, e.x, beta);
+      }
       fe_cneg<F>(e.y, (pos ^ sneg) ^ 1u);              // negative digit XOR negative half-scalar
       jac_madd<F, false>(acc, acc, e);
     }
@@ -204,8 +231,8 @@ ECG_D void k256_mul_thread(Jac& r, const uint32_t* k, const Aff& P, const TabRef
   for (int half = 0; half < 2; half++) {
     uint32_t ev = half ? g2.even : g1.even;
     uint32_t sneg = half ? g2.neg : g1.neg;
-    tab.load(0, e.x, e.y);
-    if (half) F::mul(e.x, e.x, beta);
+    tab.load(0, e.x, e.y, half ? BX : 0);
+    if (half && !F::BETA_COLUMN) F::mul(e.x, e.x, beta);
     fe_cneg<F>(e.y, sneg ^ 1u);
     Jac t;
     jac_madd<F, false>(t, acc, e);

@@ -58,7 +58,9 @@ ECG_D void jac_dbl_body(typename F::JacT& r, const typename F::JacT& p) {
   } else {
     F::sqr(L, p.X);
   }
-  F::sqr(D, A);  // Y^4
+  // with F::MUL_SUB, Y^4 is only needed as the subtrahend of Y3, and mul_sub_sqr forms it unreduced there
+  constexpr bool Y3_MUL_SUB = A_IS_MINUS3 == 0 && F::MUL_SUB && !F::SQR_TRADE_DBL;
+  if constexpr (!Y3_MUL_SUB) F::sqr(D, A);  // Y^4
   if (A_IS_MINUS3 == 0 && F::SQR_TRADE_DBL) {
     // X*Y^2 = ((X + Y^2)^2 - X^2 - Y^4)/2: a squaring (36 products) plus four linear ops instead of a multiplication (64)
     F::add(t, p.X, A);
@@ -69,16 +71,21 @@ ECG_D void jac_dbl_body(typename F::JacT& r, const typename F::JacT& p) {
   } else {
     F::mul_d(T, p.X, A);  // X*Y^2
   }
-  F::mul_small(L, L, 3);
-  if constexpr (A_IS_MINUS3 == 2) {  // general a (the field policy of such a curve carries it): L = (3 X^2 + a Z^4) / 2
-    Fe z4, ca;
-    F::sqr(zz, p.Z);
-    F::sqr(z4, zz);
-    F::curve_a(ca);
-    F::mul_d(z4, z4, ca);
-    F::add(L, L, z4);
+  if constexpr (A_IS_MINUS3 == 0 && F::HALF3_ADD) {  // 3/2 X^2 = X^2 + X^2/2, no multiplier
+    F::half(t, L);
+    F::add(L, L, t);
+  } else {
+    F::mul_small(L, L, 3);
+    if constexpr (A_IS_MINUS3 == 2) {  // general a (the field policy of such a curve carries it): L = (3 X^2 + a Z^4) / 2
+      Fe z4, ca;
+      F::sqr(zz, p.Z);
+      F::sqr(z4, zz);
+      F::curve_a(ca);
+      F::mul_d(z4, z4, ca);
+      F::add(L, L, z4);
+    }
+    F::half(L, L);
   }
-  F::half(L, L);
   if (A_IS_MINUS3 == 1 && F::DBL_3M5S) {  // Y*Z = ((Y+Z)^2 - Y^2 - Z^2)/2 ; zz was computed for L
     Fe s2;
     F::add(s2, p.Y, p.Z);
@@ -93,8 +100,12 @@ ECG_D void jac_dbl_body(typename F::JacT& r, const typename F::JacT& p) {
   F::add(t, T, T);
   F::sub(r.X, r.X, t);
   F::sub(t, T, r.X);
-  F::mul_d(r.Y, L, t);
-  F::sub(r.Y, r.Y, D);
+  if constexpr (Y3_MUL_SUB) {
+    F::mul_sub_sqr(r.Y, L, t, A);  // L (T - X3) - (Y^2)^2
+  } else {
+    F::mul_d(r.Y, L, t);
+    F::sub(r.Y, r.Y, D);
+  }
 }
 
 #if defined(__CUDA_ARCH__) || defined(__CUDACC__)
@@ -184,9 +195,13 @@ ECG_D void jac_madd_body(typename F::JacT& r, const typename F::JacT& p, const t
   F::sub(t, t, V);
   F::sub(r.X, t, V);
   F::sub(t, V, r.X);
-  F::mul(t, t, R);
-  F::mul(hhh, hhh, p.Y);
-  F::sub(r.Y, t, hhh);
+  if constexpr (F::MUL_SUB) {
+    F::mul_sub(r.Y, t, R, hhh, p.Y);  // (V - X3) R - H^3 Y1
+  } else {
+    F::mul(t, t, R);
+    F::mul(hhh, hhh, p.Y);
+    F::sub(r.Y, t, hhh);
+  }
 }
 
 template <class F, int A_IS_MINUS3>

@@ -1,7 +1,7 @@
 // tools/kbench.cu — development harness: times kernel variants of the secp256k1 variable-base path on one GPU
 // and cross-checks that every variant produces identical Jacobian words.  Not part of the product or of bench.py.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -o tools/kbench tools/kbench.cu
-//   modes: kbench 20 | kbench 20 trade | kbench 20 shape | kbench 20 mem   (mem: also build with -DECG_FE_ALIGN=16 as tools/kbench_a16)
+//   modes: kbench 20 | kbench 20 lean | kbench 20 trade | kbench 20 shape | kbench 20 mem   (mem: also build with -DECG_FE_ALIGN=16 as tools/kbench_a16)
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(BLOCK, MINBLK) kb_varbase_sync(size_t n, uint3
   make_inputs(k, P, cidx);
   Jac r;
   size_t slot = ((size_t)blockIdx.x % (132 * 8)) * BLOCK;
-  TabRef tab{gtab + slot * 128 + threadIdx.x, (uint32_t)BLOCK};
+  K256TabRef<F> tab{gtab + slot * (F::BETA_COLUMN ? 192 : 128) + threadIdx.x, (uint32_t)BLOCK};
   k256_mul_thread<F, LEVEL>(r, k, P, tab);
   if (idx >= n) return;
   for (int w = 0; w < 8; w++) {
@@ -548,6 +548,18 @@ int main(int argc, char** argv) {
       runp_sync<FpP256T<513>, 256, 2, 2>("p256 sync2 inline (256,2)", n, jac, gtab);
       runp_sync<FpP256T<513>, 512, 1, 2>("p256 sync2 inline (512,1)", n, jac, gtab);
       runp_sync<FpP256T<1537>, 512, 1, 2>("p256 sync2 inline 3M+5S (512,1)", n, jac, gtab);
+    }
+    return 0;
+  }
+  if (argc > 2 && !strcmp(argv[2], "lean")) {  // multiplier work removed from the production body (OPT bits 13-15), then the trades
+    for (int round = 0; round < 3; round++) {
+      run_sync<FpK256T<1>, 256, 2, 1>("v1     parent production (256,2)", n, jac, gtab);
+      run_sync<FpK256T<8193>, 256, 2, 1>("v8193  + beta column     (256,2)", n, jac, gtab);
+      run_sync<FpK256T<24577>, 256, 2, 1>("v24577 + 3/2 X^2 on ALU  (256,2)", n, jac, gtab);
+      run_sync<FpK256T<57345>, 256, 2, 1>("v57345 + Y3 mul_sub      (256,2)", n, jac, gtab);
+      run_sync<FpK256T<57409>, 256, 2, 1>("v57409 + dbl 2M+5S       (256,2)", n, jac, gtab);
+      run_sync<FpK256T<57473>, 256, 2, 1>("v57473 + madd 7M+4S      (256,2)", n, jac, gtab);
+      run_sync<FpK256T<57537>, 256, 2, 1>("v57537 + both trades     (256,2)", n, jac, gtab);
     }
     return 0;
   }
