@@ -13,12 +13,14 @@
 
 // This file is compiled once per curve group (-DECG_TU=0..6) so that the groups build in parallel and the kernels of
 // the headline curves keep their own translation unit:
-//   ECG_TU 0: secp256k1, P-256, P-384 + every extern "C" entry (entries for other curves forward to their group)
+//   ECG_TU 0: secp256k1, P-256, P-384 + the extern "C" entries that take an ecg_curve (calls for the curves of groups
+//             1-4 forward to their group)
 //   ECG_TU 1: sm2, brainpoolP256r1/t1, bign-curve256v1 (8 limbs)   ECG_TU 2: brainpoolP384r1/t1 (12 limbs)
 //   ECG_TU 3: P-224 (7 limbs), P-192 (6 limbs)                    ECG_TU 4: P-521 (17 limbs, 66-byte records)
 //   ECG_TU 5: X448 (Curve448, 14 limbs, 56-byte records): the host pipeline and the ladder kernel, no Weierstrass code
 //   ECG_TU 6: Ed448 (the Edwards group on the Curve448 field): verification (SHAKE256) and the group operations, the
 //             host pipelines and their kernels
+// Groups 5 and 6 take no ecg_curve and export their own extern "C" entries.
 // The groups 1-3 run the generic kernels over the generic Montgomery field policy (ecg_fe_mont.cuh).
 #ifndef ECG_TU
 #define ECG_TU 0
@@ -51,10 +53,10 @@ using namespace ecg;
 
 #define ECG_CURVE_COUNT 12
 static inline int curve_group(int c) { return c <= 2 ? 0 : c <= 6 ? 1 : c <= 8 ? 2 : c <= 10 ? 3 : 4; }
-// an entry point: extern "C" in group 0, an internal (hidden) function ecg_tuN_<name> in the other groups
+// an entry point: extern "C" in groups 0, 5 and 6, an internal (hidden) function ecg_tuN_<name> in groups 1-4
 #define ECG_CAT2(a, b) a##b
 #define ECG_CAT(a, b) ECG_CAT2(a, b)
-#if ECG_TU == 0
+#if ECG_TU == 0 || ECG_TU >= 5
 #define ECG_API(name) extern "C" ecg_status name
 #else
 #define ECG_API(name) __attribute__((visibility("hidden"))) ecg_status ECG_CAT(ECG_CAT(ECG_CAT(ecg_tu, ECG_TU), _), name)
@@ -317,6 +319,27 @@ static ecg_status copy_back(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, uint8
   if (oinf) CU_TRY(ctx, cudaMemcpyAsync(oinf + off, dp.oinf, cnt, cudaMemcpyDeviceToHost, L.s()));
   return ECG_OK;
 }
+#if ECG_TU == 0 || ECG_TU == 4 || ECG_TU == 6  // hash to curve, Ed448 verification
+// Messages of elements [off, off+cnt) of a (msgs, offsets) buffer for a kernel: in host mode the byte range
+// msgs[offsets[off] .. offsets[off+cnt]) and the cnt + 1 offsets are copied into the lane's slots `mslot` / `oslot`, and
+// *base = offsets[off] is what the kernel subtracts from the offsets; in device-pointer mode the caller's buffers, base 0.
+static ecg_status stage_msgs(ecg_ctx* ctx, Lane& L, int mslot, int oslot, const uint8_t* msgs, const uint64_t* offsets, size_t off,
+                             size_t cnt, const uint8_t** dmsgs, const uint64_t** doffs, uint64_t* base) {
+  *dmsgs = msgs;
+  *doffs = offsets + off;
+  *base = 0;
+  if (ctx->devptr()) return ECG_OK;
+  *base = offsets[off];
+  const uint64_t total = offsets[off + cnt] - *base;
+  ST_TRY(ensure(ctx, L, mslot, (size_t)total + 16));
+  ST_TRY(ensure(ctx, L, oslot, (cnt + 1) * 8));
+  if (total) CU_TRY(ctx, cudaMemcpyAsync(L.buf[mslot], msgs + *base, (size_t)total, cudaMemcpyHostToDevice, L.s()));
+  CU_TRY(ctx, cudaMemcpyAsync(L.buf[oslot], offsets + off, (cnt + 1) * 8, cudaMemcpyHostToDevice, L.s()));
+  *dmsgs = (const uint8_t*)L.buf[mslot];
+  *doffs = (const uint64_t*)L.buf[oslot];
+  return ECG_OK;
+}
+#endif
 static ecg_status begin_lane(ecg_ctx* ctx, Lane& L) {
   if (L.used) return ECG_OK;
   CU_TRY(ctx, cudaMemsetAsync(L.status, 0, 4, L.s()));
@@ -549,8 +572,6 @@ static size_t vb_minblk(ecg_curve c) {
   return c == ECG_SECP256K1 ? K_MINBLK : c == ECG_NISTP256 ? P_MINBLK : c == ECG_NISTP384 ? Q_MINBLK : (flimbs(c) > 12 ? 2 : flimbs(c) > 8 ? 3 : 4);
 }
 static size_t vb_tab_words(ecg_curve c) { return c == ECG_SECP256K1 ? K_TAB_WORDS : 8 * 3 * flimbs(c); }
-
-static size_t wave_elems(const DevState& d, ecg_curve curve) { return (size_t)d.sm_count * vb_minblk(curve) * vb_block(curve); }
 
 // per-block window-table slots for a launch of n elements
 static ecg_status ensure_tab(ecg_ctx* ctx, Lane& L, ecg_curve curve, size_t n) {
@@ -1035,50 +1056,50 @@ static std::vector<Shard> chunk_schedule(size_t cnt, size_t wave) {
   return v;
 }
 
-#if ECG_TU < 5
-static ecg_status run_batch_inner(ecg_ctx* ctx, const BatchOp& op, size_t n) {
+// The batch split of every per-element entry.  prep(d) runs once on each device that has elements, before its first
+// chunk (fixed-base tables); chunk(d, L, off, cnt) enqueues elements [off, off+cnt) on lane L of device d.  Device-pointer
+// mode runs DEV_CHUNK pieces on lane 0 of device 0.  Host mode shards the batch over the devices, cuts each shard into
+// whole waves (per_sm = resident blocks x block size of the chunk's dominant kernel) and runs chunk c of every device on
+// lane c & 1, so that copies and kernels of different chunks overlap.  Returns finish() or the first error.
+template <class Prep, class Chunk>
+static ecg_status run_chunked(ecg_ctx* ctx, size_t n, size_t per_sm, Prep prep, Chunk chunk) {
   std::vector<Shard> shards = make_shards(n, ctx->devs.size());
-  bool need_table = (op.kind == BatchOp::MULGEN && !(ctx->flags & ECG_FLAG_CONSTTIME)) || op.kind == BatchOp::MULGENADD ||
-                    op.kind == BatchOp::SCHNORR || op.kind == BatchOp::ECDSA || op.kind == BatchOp::RECOVER;
-  for (size_t i = 0; i < ctx->devs.size(); i++) {
+  for (size_t i = 0; i < shards.size(); i++) {
     if (shards[i].cnt == 0) continue;
-    DevState& d = ctx->devs[i];
-    CU_TRY(ctx, cudaSetDevice(d.dev));
-    if (need_table) {
-      ecg_status st = ensure_fb_table(ctx, d, op.curve);
-      if (st != ECG_OK) return fail(ctx, st);
-    }
+    CU_TRY(ctx, cudaSetDevice(ctx->devs[i].dev));
+    ST_TRY(prep(ctx->devs[i]));
   }
   if (ctx->devptr()) {
     DevState& d = ctx->devs[0];
-    for (size_t lo = 0; lo < n; lo += DEV_CHUNK) {
-      ecg_status st = run_chunk(ctx, d, d.lane[0], op, lo, std::min(DEV_CHUNK, n - lo));
-      if (st != ECG_OK) return fail(ctx, st);
-    }
+    for (size_t lo = 0; lo < n; lo += DEV_CHUNK) ST_TRY(chunk(d, d.lane[0], lo, std::min(DEV_CHUNK, n - lo)));
     return finish(ctx);
   }
-  // host mode: interleave chunks across devices and lanes so copies and kernels of different chunks overlap
   std::vector<std::vector<Shard>> sched(shards.size());
   size_t maxchunks = 0;
   for (size_t i = 0; i < shards.size(); i++) {
-    sched[i] = chunk_schedule(shards[i].cnt, wave_elems(ctx->devs[i], op.curve));
+    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * per_sm);
     maxchunks = std::max(maxchunks, sched[i].size());
   }
   for (size_t c = 0; c < maxchunks; c++) {
-    for (size_t i = 0; i < ctx->devs.size(); i++) {
+    for (size_t i = 0; i < shards.size(); i++) {
       if (c >= sched[i].size()) continue;
       DevState& d = ctx->devs[i];
       CU_TRY(ctx, cudaSetDevice(d.dev));
-      ecg_status st = run_chunk(ctx, d, d.lane[c & 1], op, shards[i].off + sched[i][c].off, sched[i][c].cnt);
-      if (st != ECG_OK) return fail(ctx, st);
+      ST_TRY(chunk(d, d.lane[c & 1], shards[i].off + sched[i][c].off, sched[i][c].cnt));
     }
   }
   return finish(ctx);
 }
 
+#if ECG_TU < 5
 // every error exit (including CUDA failures inside finish()) leaves the lanes reset: fail() is idempotent
 static ecg_status run_batch(ecg_ctx* ctx, const BatchOp& op, size_t n) {
-  ecg_status st = run_batch_inner(ctx, op, n);
+  const bool need_table = (op.kind == BatchOp::MULGEN && !(ctx->flags & ECG_FLAG_CONSTTIME)) || op.kind == BatchOp::MULGENADD ||
+                          op.kind == BatchOp::SCHNORR || op.kind == BatchOp::ECDSA || op.kind == BatchOp::RECOVER;
+  ecg_status st = run_chunked(
+      ctx, n, vb_minblk(op.curve) * vb_block(op.curve),
+      [&](DevState& d) { return need_table ? ensure_fb_table(ctx, d, op.curve) : ECG_OK; },
+      [&](DevState& d, Lane& L, size_t off, size_t cnt) { return run_chunk(ctx, d, L, op, off, cnt); });
   return st == ECG_OK ? st : fail(ctx, st);
 }
 
@@ -1992,27 +2013,20 @@ static ecg_status h2c_run(ecg_ctx* ctx, ecg_curve curve, size_t n, const uint8_t
   ST_TRY(begin_lane(ctx, L));
   ST_TRY(ensure(ctx, L, B_A, 256));
   CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_A], dst_prime, dpl, cudaMemcpyHostToDevice, L.s()));  // pageable, <= 256 bytes: staged by the driver
-  const uint8_t* dmsgs = msgs;
-  const uint64_t* doffs = offsets;
-  uint64_t base = 0;
   if (!ctx->devptr()) {
-    base = offsets[0];
-    const uint64_t total = offsets[n] - base;
     for (size_t i = 0; i < n; i++)
       if (offsets[i + 1] < offsets[i]) {
         ctx->err = "hash_to_curve: message offsets must be non-decreasing";
         return ECG_EINVAL;
       }
-    ST_TRY(ensure(ctx, L, B_P, (size_t)total + 16));
-    ST_TRY(ensure(ctx, L, B_K, (n + 1) * 8));
-    if (total) CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_P], msgs + base, (size_t)total, cudaMemcpyHostToDevice, L.s()));
-    CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_K], offsets, (n + 1) * 8, cudaMemcpyHostToDevice, L.s()));
-    dmsgs = (const uint8_t*)L.buf[B_P];
-    doffs = (const uint64_t*)L.buf[B_K];
   } else if (reinterpret_cast<uintptr_t>(offsets) & 7) {
     ctx->err = "device pointer (offsets) not 8-byte aligned";
     return ECG_EINVAL;
   }
+  const uint8_t* dmsgs;
+  const uint64_t* doffs;
+  uint64_t base;
+  ST_TRY(stage_msgs(ctx, L, B_P, B_K, msgs, offsets, 0, n, &dmsgs, &doffs, &base));
   const uint8_t* dprime = (const uint8_t*)L.buf[B_A];
   const size_t fb = fbytes(curve);
   DevPtrs dp;
@@ -2154,14 +2168,8 @@ extern "C" ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double*
 #endif  // ECG_TU == 0
 #endif  // ECG_TU < 5
 
-// ---- X448 (ecg_x448.cuh): group 5 holds the kernel; the public symbol (group 0) forwards there -------------------------
-#if ECG_TU == 0
-__attribute__((visibility("hidden"))) ecg_status ecg_tu5_ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56,
-                                                                         uint8_t* ok);
-extern "C" ecg_status ecg_x448_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok) {
-  return ecg_tu5_ecg_x448_batch(ctx, n, k56, u56, out56, ok);
-}
-#elif ECG_TU == 5
+// ---- X448 (ecg_x448.cuh): group 5 -------------------------------------------------------------------------------------
+#if ECG_TU == 5
 // one chunk: stage the scalars and u values, one ladder per thread, copy the results and the low-order flags back
 static ecg_status x448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, const uint8_t* k56, const uint8_t* u56, uint8_t* out56,
                              uint8_t* ok) {
@@ -2176,32 +2184,6 @@ static ecg_status x448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, cons
   DOM_END(ctx, L);
   return copy_back(ctx, L, off, cnt, out56, 56, ok, dp);
 }
-// the batch split of run_batch_inner: device-pointer mode in DEV_CHUNK pieces on lane 0; host mode sharded over the
-// devices and cut into whole waves of the ladder kernel, alternating lanes so that copies overlap the kernels
-static ecg_status x448_run(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok) {
-  if (ctx->devptr()) {
-    DevState& d = ctx->devs[0];
-    CU_TRY(ctx, cudaSetDevice(d.dev));
-    for (size_t lo = 0; lo < n; lo += DEV_CHUNK) ST_TRY(x448_chunk(ctx, d.lane[0], lo, std::min(DEV_CHUNK, n - lo), k56, u56, out56, ok));
-    return finish(ctx);
-  }
-  std::vector<Shard> shards = make_shards(n, ctx->devs.size());
-  std::vector<std::vector<Shard>> sched(shards.size());
-  size_t maxchunks = 0;
-  for (size_t i = 0; i < shards.size(); i++) {
-    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * X448_MINBLK * X448_BLOCK);
-    maxchunks = std::max(maxchunks, sched[i].size());
-  }
-  for (size_t c = 0; c < maxchunks; c++) {
-    for (size_t i = 0; i < ctx->devs.size(); i++) {
-      if (c >= sched[i].size()) continue;
-      DevState& d = ctx->devs[i];
-      CU_TRY(ctx, cudaSetDevice(d.dev));
-      ST_TRY(x448_chunk(ctx, d.lane[c & 1], shards[i].off + sched[i][c].off, sched[i][c].cnt, k56, u56, out56, ok));
-    }
-  }
-  return finish(ctx);
-}
 ECG_API(ecg_x448_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* u56, uint8_t* out56, uint8_t* ok) {
   if (!ctx) return ECG_EINVAL;
   if (n == 0) return ECG_OK;
@@ -2209,21 +2191,15 @@ ECG_API(ecg_x448_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_
     ctx->err = "ecg_x448_batch: null pointer";
     return ECG_EINVAL;
   }
-  ecg_status st = x448_run(ctx, n, k56, u56, out56, ok);
+  ecg_status st = run_chunked(
+      ctx, n, X448_MINBLK * X448_BLOCK, [](DevState&) { return ECG_OK; },
+      [&](DevState&, Lane& L, size_t off, size_t cnt) { return x448_chunk(ctx, L, off, cnt, k56, u56, out56, ok); });
   return st == ECG_OK ? st : fail(ctx, st);
 }
 #endif
 
-// ---- Ed448 verification (ecg_ed448.cuh): group 6 holds the kernel; the public symbol (group 0) forwards there ----------
-#if ECG_TU == 0
-__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114,
-                                                                                 const uint8_t* msgs, const uint64_t* offsets, const uint8_t* context,
-                                                                                 size_t context_len, int prehashed, uint8_t* valid);
-extern "C" ecg_status ecg_ed448_verify_batch(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs,
-                                             const uint64_t* offsets, const uint8_t* context, size_t context_len, int prehashed, uint8_t* valid) {
-  return ecg_tu6_ecg_ed448_verify_batch(ctx, n, pk57, sig114, msgs, offsets, context, context_len, prehashed, valid);
-}
-#elif ECG_TU == 6
+// ---- Ed448 verification (ecg_ed448.cuh): group 6 ------------------------------------------------------------------------
+#if ECG_TU == 6
 // one chunk [off, off + cnt): stage the keys, the signatures, the chunk's own byte range of the messages and its offsets
 // (the kernel subtracts the range's start), one verification per thread, copy the verdicts back
 static ecg_status ed448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs,
@@ -2232,19 +2208,10 @@ static ecg_status ed448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, con
   ST_TRY(begin_lane(ctx, L));
   ST_TRY(stage_in(ctx, L, B_K, pk57, off, cnt, 57, &dp.k));
   ST_TRY(stage_in(ctx, L, B_P, sig114, off, cnt, 114, &dp.p));
-  const uint8_t* dmsgs = msgs;
-  const uint64_t* doffs = offsets + off;
-  uint64_t base = 0;
-  if (!ctx->devptr()) {
-    base = offsets[off];
-    const uint64_t total = offsets[off + cnt] - base;
-    ST_TRY(ensure(ctx, L, B_A, (size_t)total + 16));
-    ST_TRY(ensure(ctx, L, B_X, (cnt + 1) * 8));
-    if (total) CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_A], msgs + base, (size_t)total, cudaMemcpyHostToDevice, L.s()));
-    CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_X], offsets + off, (cnt + 1) * 8, cudaMemcpyHostToDevice, L.s()));
-    dmsgs = (const uint8_t*)L.buf[B_A];
-    doffs = (const uint64_t*)L.buf[B_X];
-  }
+  const uint8_t* dmsgs;
+  const uint64_t* doffs;
+  uint64_t base;
+  ST_TRY(stage_msgs(ctx, L, B_A, B_X, msgs, offsets, off, cnt, &dmsgs, &doffs, &base));
   ST_TRY(stage_out(ctx, L, off, cnt, valid, 1, nullptr, dp));
   DOM_BEGIN(ctx, L);
   ed448_verify_kernel<FpEd448, ED448_BLOCK, ED448_MINBLK><<<grid_for(cnt, ED448_BLOCK), ED448_BLOCK, 0, L.s()>>>(dp.k, dp.p, dmsgs, doffs, base, cnt,
@@ -2280,34 +2247,6 @@ static ecg_status ed448_check_offsets(ecg_ctx* ctx, size_t n, const uint64_t* of
   }
   return ECG_OK;
 }
-// the batch split of x448_run: device-pointer mode in DEV_CHUNK pieces on lane 0; host mode sharded over the devices and
-// cut into whole waves of the kernel, alternating lanes so that copies overlap the kernels
-static ecg_status ed448_run(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs, const uint64_t* offsets,
-                            const Ed448Dom& dom, uint8_t* valid) {
-  if (ctx->devptr()) {
-    DevState& d = ctx->devs[0];
-    CU_TRY(ctx, cudaSetDevice(d.dev));
-    for (size_t lo = 0; lo < n; lo += DEV_CHUNK)
-      ST_TRY(ed448_chunk(ctx, d.lane[0], lo, std::min(DEV_CHUNK, n - lo), pk57, sig114, msgs, offsets, dom, valid));
-    return finish(ctx);
-  }
-  std::vector<Shard> shards = make_shards(n, ctx->devs.size());
-  std::vector<std::vector<Shard>> sched(shards.size());
-  size_t maxchunks = 0;
-  for (size_t i = 0; i < shards.size(); i++) {
-    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * ED448_MINBLK * ED448_BLOCK);
-    maxchunks = std::max(maxchunks, sched[i].size());
-  }
-  for (size_t c = 0; c < maxchunks; c++) {
-    for (size_t i = 0; i < ctx->devs.size(); i++) {
-      if (c >= sched[i].size()) continue;
-      DevState& d = ctx->devs[i];
-      CU_TRY(ctx, cudaSetDevice(d.dev));
-      ST_TRY(ed448_chunk(ctx, d.lane[c & 1], shards[i].off + sched[i][c].off, sched[i][c].cnt, pk57, sig114, msgs, offsets, dom, valid));
-    }
-  }
-  return finish(ctx);
-}
 ECG_API(ecg_ed448_verify_batch)(ecg_ctx* ctx, size_t n, const uint8_t* pk57, const uint8_t* sig114, const uint8_t* msgs,
                                 const uint64_t* offsets, const uint8_t* context, size_t context_len, int prehashed, uint8_t* valid) {
   if (!ctx) return ECG_EINVAL;
@@ -2329,28 +2268,15 @@ ECG_API(ecg_ed448_verify_batch)(ecg_ctx* ctx, size_t n, const uint8_t* pk57, con
   dom.b[9] = (uint8_t)context_len;
   if (context_len) memcpy(dom.b + 10, context, context_len);
   dom.len = (uint32_t)(10 + context_len);
-  st = ed448_run(ctx, n, pk57, sig114, msgs, offsets, dom, valid);
+  st = run_chunked(ctx, n, ED448_MINBLK * ED448_BLOCK, [](DevState&) { return ECG_OK; }, [&](DevState&, Lane& L, size_t off, size_t cnt) {
+    return ed448_chunk(ctx, L, off, cnt, pk57, sig114, msgs, offsets, dom, valid);
+  });
   return st == ECG_OK ? st : fail(ctx, st);
 }
 #endif
 
-// ---- Ed448 group operations (ecg_ed448_group.cuh): group 6 holds the kernels; the public symbols (group 0) forward there --
-#if ECG_TU == 0
-__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_mul_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57,
-                                                                              uint8_t* out57);
-__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57);
-__attribute__((visibility("hidden"))) ecg_status ecg_tu6_ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57,
-                                                                            uint8_t* out57);
-extern "C" ecg_status ecg_ed448_mul_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
-  return ecg_tu6_ecg_ed448_mul_batch(ctx, n, k57, P57, out57);
-}
-extern "C" ecg_status ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57) {
-  return ecg_tu6_ecg_ed448_mul_gen_batch(ctx, n, k57, out57);
-}
-extern "C" ecg_status ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
-  return ecg_tu6_ecg_ed448_lincomb(ctx, n, k57, P57, out57);
-}
-#elif ECG_TU == 6
+// ---- Ed448 group operations (ecg_ed448_group.cuh): group 6 --------------------------------------------------------------
+#if ECG_TU == 6
 static const size_t ED448G_PT = 56 * 4;  // bytes of one extended point
 
 // [k_i] P_i (p57 == nullptr: P_i = B) for cnt elements into ext (SoA, stride cnt); base = index of the first element
@@ -2448,39 +2374,6 @@ static ecg_status ed448g_chunk(ecg_ctx* ctx, DevState& d, Lane& L, bool gen, siz
   DOM_END(ctx, L);
   ST_TRY(ed448g_norm<false>(ctx, L, ext, cnt, dp.out));
   return copy_back(ctx, L, off, cnt, out57, 57, nullptr, dp);
-}
-// the batch split of x448_run: device-pointer mode in DEV_CHUNK pieces on lane 0; host mode sharded over the devices and
-// cut into whole waves of the kernel, alternating lanes so that copies overlap the kernels
-static ecg_status ed448g_run(ecg_ctx* ctx, bool gen, size_t n, const uint8_t* k57, const uint8_t* p57, uint8_t* out57) {
-  const bool table = gen && !(ctx->flags & ECG_FLAG_CONSTTIME);
-  const size_t minblk = table ? ED448G_FB_MINBLK : ED448G_MINBLK;
-  if (ctx->devptr()) {
-    DevState& d = ctx->devs[0];
-    CU_TRY(ctx, cudaSetDevice(d.dev));
-    if (table) ST_TRY(ensure_ed448_table(ctx, d));
-    for (size_t lo = 0; lo < n; lo += DEV_CHUNK) ST_TRY(ed448g_chunk(ctx, d, d.lane[0], gen, lo, std::min(DEV_CHUNK, n - lo), k57, p57, out57));
-    return finish(ctx);
-  }
-  std::vector<Shard> shards = make_shards(n, ctx->devs.size());
-  std::vector<std::vector<Shard>> sched(shards.size());
-  size_t maxchunks = 0;
-  for (size_t i = 0; i < shards.size(); i++) {
-    if (table && shards[i].cnt) {
-      CU_TRY(ctx, cudaSetDevice(ctx->devs[i].dev));
-      ST_TRY(ensure_ed448_table(ctx, ctx->devs[i]));
-    }
-    sched[i] = chunk_schedule(shards[i].cnt, (size_t)ctx->devs[i].sm_count * minblk * ED448G_BLOCK);
-    maxchunks = std::max(maxchunks, sched[i].size());
-  }
-  for (size_t c = 0; c < maxchunks; c++) {
-    for (size_t i = 0; i < ctx->devs.size(); i++) {
-      if (c >= sched[i].size()) continue;
-      DevState& d = ctx->devs[i];
-      CU_TRY(ctx, cudaSetDevice(d.dev));
-      ST_TRY(ed448g_chunk(ctx, d, d.lane[c & 1], gen, shards[i].off + sched[i][c].off, sched[i][c].cnt, k57, p57, out57));
-    }
-  }
-  return finish(ctx);
 }
 // the sum of n extended points (SoA in a, stride n), 32 to 1 per pass, ping-ponging through b; the result's word w goes
 // to dst[w * dst_stride]
@@ -2581,7 +2474,9 @@ ECG_API(ecg_ed448_mul_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k57, const u
     ctx->err = "ecg_ed448_mul_batch: null pointer";
     return ECG_EINVAL;
   }
-  ecg_status st = ed448g_run(ctx, false, n, k57, P57, out57);
+  ecg_status st = run_chunked(ctx, n, ED448G_MINBLK * ED448G_BLOCK, [](DevState&) { return ECG_OK; }, [&](DevState& d, Lane& L, size_t off, size_t cnt) {
+    return ed448g_chunk(ctx, d, L, false, off, cnt, k57, P57, out57);
+  });
   return st == ECG_OK ? st : fail(ctx, st);
 }
 ECG_API(ecg_ed448_mul_gen_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k57, uint8_t* out57) {
@@ -2591,7 +2486,10 @@ ECG_API(ecg_ed448_mul_gen_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k57, uin
     ctx->err = "ecg_ed448_mul_gen_batch: null pointer";
     return ECG_EINVAL;
   }
-  ecg_status st = ed448g_run(ctx, true, n, k57, nullptr, out57);
+  const bool table = !(ctx->flags & ECG_FLAG_CONSTTIME);  // ECG_FLAG_CONSTTIME: the variable-base routine on B
+  ecg_status st = run_chunked(
+      ctx, n, (table ? ED448G_FB_MINBLK : ED448G_MINBLK) * ED448G_BLOCK, [&](DevState& d) { return table ? ensure_ed448_table(ctx, d) : ECG_OK; },
+      [&](DevState& d, Lane& L, size_t off, size_t cnt) { return ed448g_chunk(ctx, d, L, true, off, cnt, k57, nullptr, out57); });
   return st == ECG_OK ? st : fail(ctx, st);
 }
 ECG_API(ecg_ed448_lincomb)(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
