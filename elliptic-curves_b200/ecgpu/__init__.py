@@ -603,6 +603,15 @@ class Engine:
     def lincomb_ptr(self, curve, n, k, P_xy, P_inf, out_xy, out_inf):
         self._check(self.lib.ecg_lincomb(self._ctx, CURVE_IDS[curve], n, _ptr(k), _ptr(P_xy), _ptr(P_inf), _ptr(out_xy), _ptr(out_inf)))
 
+    def mul_batch_x_ptr(self, curve, n, k, P_xy, P_inf, out_x, out_inf):
+        self._check(self.lib.ecg_mul_batch_x(self._ctx, CURVE_IDS[curve], n, _ptr(k), _ptr(P_xy), _ptr(P_inf), _ptr(out_x), _ptr(out_inf)))
+
+    def batch_normalize_ptr(self, curve, n, xyz, out_xy, out_inf):
+        self._check(self.lib.ecg_batch_normalize(self._ctx, CURVE_IDS[curve], n, _ptr(xyz), _ptr(out_xy), _ptr(out_inf)))
+
+    def batch_normalize_hom_ptr(self, curve, n, xyz, out_xy, out_inf):
+        self._check(self.lib.ecg_batch_normalize_hom(self._ctx, CURVE_IDS[curve], n, _ptr(xyz), _ptr(out_xy), _ptr(out_inf)))
+
     def point_sum_ptr(self, curve, m, xyz, out_xy, out_inf):
         """sum of m Jacobian points (m*96 bytes in device memory, e.g. an all_gather receive buffer) -> affine, on the device"""
         self._check(self.lib.ecg_point_sum(self._ctx, CURVE_IDS[curve], m, _ptr(xyz), _ptr(out_xy), _ptr(out_inf)))
