@@ -91,6 +91,21 @@ struct Shake256 {
 #pragma unroll
     for (int i = 0; i < N; i++) out[i] = (uint8_t)(s[i >> 3] >> (8 * (i & 7)));
   }
+  // pad (0x1F ... 0x80) and squeeze N bytes of any length: one more permutation before every further 136-byte block
+  template <int N>
+  ECG_D void finish_long(uint8_t* out) {
+    buf[pos++] = 0x1F;
+#pragma unroll 1
+    while (pos < 136) buf[pos++] = 0;
+    buf[135] |= 0x80;
+    absorb_block();
+#pragma unroll 1
+    for (int i = 0; i < N; i++) {
+      const int j = i % 136;
+      if (i && j == 0) keccak_f1600(s);
+      out[i] = (uint8_t)(s[j >> 3] >> (8 * (j & 7)));
+    }
+  }
 };
 
 }  // namespace ecg

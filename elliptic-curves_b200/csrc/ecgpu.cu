@@ -18,8 +18,8 @@
 //   ECG_TU 1: sm2, brainpoolP256r1/t1, bign-curve256v1 (8 limbs)   ECG_TU 2: brainpoolP384r1/t1 (12 limbs)
 //   ECG_TU 3: P-224 (7 limbs), P-192 (6 limbs)                    ECG_TU 4: P-521 (17 limbs, 66-byte records)
 //   ECG_TU 5: X448 (Curve448, 14 limbs, 56-byte records): the host pipeline and the ladder kernel, no Weierstrass code
-//   ECG_TU 6: Ed448 (the Edwards group on the Curve448 field): verification (SHAKE256) and the group operations, the
-//             host pipelines and their kernels
+//   ECG_TU 6: Ed448 (the Edwards group on the Curve448 field): verification (SHAKE256) and the group operations, and
+//             Decaf448 on the same point layer; the host pipelines and their kernels
 // Groups 5 and 6 take no ecg_curve and export their own extern "C" entries.
 // The groups 1-3 run the generic kernels over the generic Montgomery field policy (ecg_fe_mont.cuh).
 #ifndef ECG_TU
@@ -31,7 +31,7 @@
 #if ECG_TU == 5
 #include "ecg_x448.cuh"
 #else
-#include "ecg_ed448_group.cuh"
+#include "ecg_decaf448.cuh"
 #endif
 using namespace ecg;
 // the status flags of ecg_kernels.cuh that finish() reads; every 56-byte string is a valid X448 input, and an Ed448
@@ -2220,13 +2220,13 @@ static ecg_status ed448_chunk(ecg_ctx* ctx, Lane& L, size_t off, size_t cnt, con
   DOM_END(ctx, L);
   return copy_back(ctx, L, off, cnt, valid, 1, nullptr, dp);
 }
-// offsets[0..n] must not decrease (in device-pointer mode they are read back first: 8 (n + 1) bytes)
-static ecg_status ed448_check_offsets(ecg_ctx* ctx, size_t n, const uint64_t* offsets, const uint8_t* msgs) {
+// offsets[0..n] must not decrease (in device-pointer mode they are read back first: 8 (n + 1) bytes); `who` names the entry
+static ecg_status ed448_check_offsets(ecg_ctx* ctx, const char* who, size_t n, const uint64_t* offsets, const uint8_t* msgs) {
   std::vector<uint64_t> host;
   const uint64_t* o = offsets;
   if (ctx->devptr()) {
     if (reinterpret_cast<uintptr_t>(offsets) & 7) {
-      ctx->err = "ecg_ed448_verify_batch: device pointer (offsets) not 8-byte aligned";
+      ctx->err = std::string(who) + ": device pointer (offsets) not 8-byte aligned";
       return ECG_EINVAL;
     }
     Lane& L = ctx->devs[0].lane[0];
@@ -2238,11 +2238,11 @@ static ecg_status ed448_check_offsets(ecg_ctx* ctx, size_t n, const uint64_t* of
   }
   for (size_t i = 0; i < n; i++)
     if (o[i + 1] < o[i]) {
-      ctx->err = "ecg_ed448_verify_batch: message offsets must be non-decreasing";
+      ctx->err = std::string(who) + ": message offsets must be non-decreasing";
       return ECG_EINVAL;
     }
   if (!msgs && o[n] != o[0]) {
-    ctx->err = "ecg_ed448_verify_batch: null message buffer";
+    ctx->err = std::string(who) + ": null message buffer";
     return ECG_EINVAL;
   }
   return ECG_OK;
@@ -2259,7 +2259,7 @@ ECG_API(ecg_ed448_verify_batch)(ecg_ctx* ctx, size_t n, const uint8_t* pk57, con
     ctx->err = "ecg_ed448_verify_batch: null pointer";
     return ECG_EINVAL;
   }
-  ecg_status st = ed448_check_offsets(ctx, n, offsets, msgs);
+  ecg_status st = ed448_check_offsets(ctx, "ecg_ed448_verify_batch", n, offsets, msgs);
   if (st != ECG_OK) return st;
   // dom4 = "SigEd448" || phflag || len(ctx) || ctx (RFC 8032 section 2; sign.rs:105, verifying_key.rs:290-303)
   Ed448Dom dom;
@@ -2389,9 +2389,12 @@ static ecg_status ed448g_reduce(ecg_ctx* ctx, Lane& L, uint32_t* a, uint32_t* b,
   LAUNCHED(ctx);
   return ECG_OK;
 }
+static ecg_status decaf448_launch_mul(ecg_ctx* ctx, Lane& L, const uint8_t* k56, const uint8_t* p56, size_t cnt, size_t base, uint32_t* ext);
+static ecg_status decaf448_launch_encode(ecg_ctx* ctx, Lane& L, const uint32_t* ext, size_t n, uint8_t* out56);
 // sum of [k_i] P_i over [off, off + cnt) on device d (lane 0), in pieces of at most DEV_CHUNK terms: each piece's
-// products are summed into one slot of B_V1, the slots into B_V2 (one extended point, *res)
-static ecg_status ed448g_lincomb_shard(ecg_ctx* ctx, DevState& d, size_t off, size_t cnt, const uint8_t* k57, const uint8_t* p57,
+// products are summed into one slot of B_V1, the slots into B_V2 (one extended point, *res).  decaf: 56-byte Decaf448
+// records (decaf448_mul_kernel) instead of 57-byte Ed448 records.
+static ecg_status ed448g_lincomb_shard(ecg_ctx* ctx, DevState& d, bool decaf, size_t off, size_t cnt, const uint8_t* k57, const uint8_t* p57,
                                        uint32_t** res) {
   Lane& L = d.lane[0];
   ST_TRY(begin_lane(ctx, L));
@@ -2404,10 +2407,14 @@ static ecg_status ed448g_lincomb_shard(ecg_ctx* ctx, DevState& d, size_t off, si
   for (size_t pc = 0; pc < pieces; pc++) {
     const size_t lo = off + pc * DEV_CHUNK, m = std::min(DEV_CHUNK, off + cnt - lo);
     DevPtrs dp;
-    ST_TRY(stage_in(ctx, L, B_K, k57, lo, m, 57, &dp.k));
-    ST_TRY(stage_in(ctx, L, B_P, p57, lo, m, 57, &dp.p));
+    const size_t rec = decaf ? 56 : 57;
+    ST_TRY(stage_in(ctx, L, B_K, k57, lo, m, rec, &dp.k));
+    ST_TRY(stage_in(ctx, L, B_P, p57, lo, m, rec, &dp.p));
     DOM_BEGIN(ctx, L);
-    ST_TRY(ed448g_launch_mul(ctx, L, dp.k, dp.p, m, lo, (uint32_t*)L.buf[B_JAC]));
+    if (decaf)
+      ST_TRY(decaf448_launch_mul(ctx, L, dp.k, dp.p, m, lo, (uint32_t*)L.buf[B_JAC]));
+    else
+      ST_TRY(ed448g_launch_mul(ctx, L, dp.k, dp.p, m, lo, (uint32_t*)L.buf[B_JAC]));
     DOM_END(ctx, L);
     ST_TRY(ed448g_reduce(ctx, L, (uint32_t*)L.buf[B_JAC], (uint32_t*)L.buf[B_JAC2], m, part + pc, pieces));
   }
@@ -2415,25 +2422,30 @@ static ecg_status ed448g_lincomb_shard(ecg_ctx* ctx, DevState& d, size_t off, si
   *res = (uint32_t*)L.buf[B_V2];
   return ECG_OK;
 }
-// one point (56 words at pt) -> the compressed record out57 (a caller pointer), on lane 0 of device d
-static ecg_status ed448g_finish_point(ecg_ctx* ctx, DevState& d, const uint32_t* pt, uint8_t* out57) {
+// one point (56 words at pt) -> the compressed record out57 (a caller pointer), on lane 0 of device d; decaf: the
+// 56-byte Decaf448 encoding
+static ecg_status ed448g_finish_point(ecg_ctx* ctx, DevState& d, bool decaf, const uint32_t* pt, uint8_t* out57) {
   Lane& L = d.lane[0];
   DevPtrs dp;
-  ST_TRY(stage_out(ctx, L, 0, 1, out57, 57, nullptr, dp));
-  ST_TRY(ed448g_norm<false>(ctx, L, pt, 1, dp.out));
-  return copy_back(ctx, L, 0, 1, out57, 57, nullptr, dp);
+  const size_t rec = decaf ? 56 : 57;
+  ST_TRY(stage_out(ctx, L, 0, 1, out57, rec, nullptr, dp));
+  if (decaf)
+    ST_TRY(decaf448_launch_encode(ctx, L, pt, 1, dp.out));
+  else
+    ST_TRY(ed448g_norm<false>(ctx, L, pt, 1, dp.out));
+  return copy_back(ctx, L, 0, 1, out57, rec, nullptr, dp);
 }
 // every device's shard is enqueued before any is waited for; the partial sums come back through pinned host memory and
 // device 0 adds them
-static ecg_status ed448g_lincomb_run(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* p57, uint8_t* out57) {
+static ecg_status ed448g_lincomb_run(ecg_ctx* ctx, bool decaf, size_t n, const uint8_t* k57, const uint8_t* p57, uint8_t* out57) {
   const size_t nd = ctx->devs.size();
   std::vector<Shard> shards = make_shards(n, nd);
   if (nd == 1) {
     DevState& d = ctx->devs[0];
     CU_TRY(ctx, cudaSetDevice(d.dev));
     uint32_t* res = nullptr;
-    ST_TRY(ed448g_lincomb_shard(ctx, d, 0, n, k57, p57, &res));
-    ST_TRY(ed448g_finish_point(ctx, d, res, out57));
+    ST_TRY(ed448g_lincomb_shard(ctx, d, decaf, 0, n, k57, p57, &res));
+    ST_TRY(ed448g_finish_point(ctx, d, decaf, res, out57));
     return finish(ctx);
   }
   for (size_t i = 0; i < nd; i++) {
@@ -2441,7 +2453,7 @@ static ecg_status ed448g_lincomb_run(ecg_ctx* ctx, size_t n, const uint8_t* k57,
     DevState& d = ctx->devs[i];
     CU_TRY(ctx, cudaSetDevice(d.dev));
     uint32_t* res = nullptr;
-    ST_TRY(ed448g_lincomb_shard(ctx, d, shards[i].off, shards[i].cnt, k57, p57, &res));
+    ST_TRY(ed448g_lincomb_shard(ctx, d, decaf, shards[i].off, shards[i].cnt, k57, p57, &res));
     CU_TRY(ctx, cudaMemcpyAsync(d.lane[0].h_point(), res, ED448G_PT, cudaMemcpyDeviceToHost, d.lane[0].s()));
   }
   ST_TRY(finish(ctx));
@@ -2464,7 +2476,7 @@ static ecg_status ed448g_lincomb_run(ecg_ctx* ctx, size_t n, const uint8_t* k57,
   ST_TRY(ensure(ctx, L, B_V2, ED448G_PT));
   CU_TRY(ctx, cudaMemcpyAsync(L.buf[B_V3], parts.data(), nd * ED448G_PT, cudaMemcpyHostToDevice, L.s()));
   ST_TRY(ed448g_reduce(ctx, L, (uint32_t*)L.buf[B_V3], (uint32_t*)L.buf[B_V4], nd, (uint32_t*)L.buf[B_V2], 1));
-  ST_TRY(ed448g_finish_point(ctx, d, (const uint32_t*)L.buf[B_V2], out57));
+  ST_TRY(ed448g_finish_point(ctx, d, decaf, (const uint32_t*)L.buf[B_V2], out57));
   return finish(ctx);
 }
 ECG_API(ecg_ed448_mul_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t* out57) {
@@ -2510,7 +2522,188 @@ ECG_API(ecg_ed448_lincomb)(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uin
     }
     return ECG_OK;
   }
-  ecg_status st = ed448g_lincomb_run(ctx, n, k57, P57, out57);
+  ecg_status st = ed448g_lincomb_run(ctx, false, n, k57, P57, out57);
   return st == ECG_OK ? st : fail(ctx, st);
+}
+#endif
+
+// ---- Decaf448 (ecg_decaf448.cuh): group 6 -------------------------------------------------------------------------------
+#if ECG_TU == 6
+// [k_i] P_i (p56 == nullptr: P_i = G0) for cnt elements into ext (SoA, stride cnt); base = index of the first element
+static ecg_status decaf448_launch_mul(ecg_ctx* ctx, Lane& L, const uint8_t* k56, const uint8_t* p56, size_t cnt, size_t base, uint32_t* ext) {
+  const bool scrub = (ctx->flags & ECG_FLAG_ZEROIZE) != 0;
+  if (ctx->flags & ECG_FLAG_CONSTTIME)
+    decaf448_mul_kernel<FpEd448, true><<<grid_for(cnt, DECAF448_BLOCK), DECAF448_BLOCK, 0, L.s()>>>(k56, p56, cnt, base, ext, L.status, scrub);
+  else
+    decaf448_mul_kernel<FpEd448, false><<<grid_for(cnt, DECAF448_BLOCK), DECAF448_BLOCK, 0, L.s()>>>(k56, p56, cnt, base, ext, L.status, scrub);
+  LAUNCHED(ctx);
+  return ECG_OK;
+}
+// n extended points (SoA in ext) -> n 56-byte encodings
+static ecg_status decaf448_launch_encode(ecg_ctx* ctx, Lane& L, const uint32_t* ext, size_t n, uint8_t* out56) {
+  decaf448_encode_kernel<FpEd448><<<grid_for(n, DECAF448_BLOCK), DECAF448_BLOCK, 0, L.s()>>>(ext, n, out56);
+  LAUNCHED(ctx);
+  return ECG_OK;
+}
+// one chunk of ecg_decaf448_mul_batch (gen = false) or ecg_decaf448_mul_gen_batch (gen = true): stage the records, one
+// scalar multiplication per thread (k G: the Ed448 fixed-base table, or under CONSTTIME the variable-base routine on
+// G0), encode, copy the records back
+static ecg_status decaf448_chunk(ecg_ctx* ctx, DevState& d, Lane& L, bool gen, size_t off, size_t cnt, const uint8_t* k56, const uint8_t* p56,
+                                 uint8_t* out56) {
+  DevPtrs dp;
+  ST_TRY(begin_lane(ctx, L));
+  ST_TRY(stage_in(ctx, L, B_K, k56, off, cnt, 56, &dp.k));
+  ST_TRY(stage_in(ctx, L, B_P, gen ? nullptr : p56, off, cnt, 56, &dp.p));
+  ST_TRY(ensure(ctx, L, B_JAC, cnt * ED448G_PT));
+  ST_TRY(stage_out(ctx, L, off, cnt, out56, 56, nullptr, dp));
+  uint32_t* ext = (uint32_t*)L.buf[B_JAC];
+  DOM_BEGIN(ctx, L);
+  if (gen && !(ctx->flags & ECG_FLAG_CONSTTIME)) {
+    decaf448_fixed_kernel<FpEd448><<<grid_for(cnt, DECAF448_BLOCK), DECAF448_BLOCK, 0, L.s()>>>(dp.k, cnt, off, d.ed448_table, ext, L.status);
+    LAUNCHED(ctx);
+  } else {
+    ST_TRY(decaf448_launch_mul(ctx, L, dp.k, dp.p, cnt, off, ext));
+  }
+  DOM_END(ctx, L);
+  ST_TRY(decaf448_launch_encode(ctx, L, ext, cnt, dp.out));
+  return copy_back(ctx, L, off, cnt, out56, 56, nullptr, dp);
+}
+ECG_API(ecg_decaf448_mul_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* P56, uint8_t* out56) {
+  if (!ctx) return ECG_EINVAL;
+  if (n == 0) return ECG_OK;
+  if (!k56 || !P56 || !out56) {
+    ctx->err = "ecg_decaf448_mul_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = run_chunked(ctx, n, DECAF448_MINBLK * DECAF448_BLOCK, [](DevState&) { return ECG_OK; },
+                              [&](DevState& d, Lane& L, size_t off, size_t cnt) { return decaf448_chunk(ctx, d, L, false, off, cnt, k56, P56, out56); });
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+ECG_API(ecg_decaf448_mul_gen_batch)(ecg_ctx* ctx, size_t n, const uint8_t* k56, uint8_t* out56) {
+  if (!ctx) return ECG_EINVAL;
+  if (n == 0) return ECG_OK;
+  if (!k56 || !out56) {
+    ctx->err = "ecg_decaf448_mul_gen_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  const bool table = !(ctx->flags & ECG_FLAG_CONSTTIME);  // the Ed448 fixed-base table, shared with ecg_ed448_mul_gen_batch
+  ecg_status st = run_chunked(
+      ctx, n, (table ? DECAF448_FB_MINBLK : DECAF448_MINBLK) * DECAF448_BLOCK, [&](DevState& d) { return table ? ensure_ed448_table(ctx, d) : ECG_OK; },
+      [&](DevState& d, Lane& L, size_t off, size_t cnt) { return decaf448_chunk(ctx, d, L, true, off, cnt, k56, nullptr, out56); });
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+ECG_API(ecg_decaf448_lincomb)(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* P56, uint8_t* out56) {
+  if (!ctx) return ECG_EINVAL;
+  if (!out56 || (n > 0 && (!k56 || !P56))) {
+    ctx->err = "ecg_decaf448_lincomb: null pointer";
+    return ECG_EINVAL;
+  }
+  if (n == 0) {  // the identity, 56 zero bytes
+    if (ctx->devptr()) {
+      CU_TRY(ctx, cudaSetDevice(ctx->devs[0].dev));
+      CU_TRY(ctx, cudaMemset(out56, 0, 56));
+    } else {
+      memset(out56, 0, 56);
+    }
+    return ECG_OK;
+  }
+  ecg_status st = ed448g_lincomb_run(ctx, true, n, k56, P56, out56);
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+// ok[i] = 1 iff CompressedDecaf::decompress accepts record i: per-record verdicts, never a refusal
+ECG_API(ecg_decaf448_check_batch)(ecg_ctx* ctx, size_t n, const uint8_t* P56, uint8_t* ok) {
+  if (!ctx) return ECG_EINVAL;
+  if (n == 0) return ECG_OK;
+  if (!P56 || !ok) {
+    ctx->err = "ecg_decaf448_check_batch: null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = run_chunked(ctx, n, DECAF448_MINBLK * DECAF448_BLOCK, [](DevState&) { return ECG_OK; }, [&](DevState&, Lane& L, size_t off, size_t cnt) {
+    DevPtrs dp;
+    ST_TRY(begin_lane(ctx, L));
+    ST_TRY(stage_in(ctx, L, B_P, P56, off, cnt, 56, &dp.p));
+    ST_TRY(stage_out(ctx, L, off, cnt, ok, 1, nullptr, dp));
+    DOM_BEGIN(ctx, L);
+    decaf448_check_kernel<FpEd448><<<grid_for(cnt, DECAF448_BLOCK), DECAF448_BLOCK, 0, L.s()>>>(dp.p, cnt, dp.out);
+    LAUNCHED(ctx);
+    DOM_END(ctx, L);
+    return copy_back(ctx, L, off, cnt, ok, 1, nullptr, dp);
+  });
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+// the suffix expand_message_xof absorbs after the message (ecg_decaf448.cuh, XofSuffix): I2OSP(len_in_bytes, 2) || DST' ||
+// I2OSP(len(DST'), 1).  A DST over 255 bytes becomes SHAKE256("H2C-OVERSIZE-DST-" || DST, 56), computed by one device
+// thread on lane 0 of device 0 (synchronously: the suffix is a kernel parameter of every chunk).  dst is non-empty.
+static ecg_status decaf448_suffix(ecg_ctx* ctx, const uint8_t* dst, size_t dst_len, uint32_t len_in_bytes, XofSuffix* sfx) {
+  memset(sfx, 0, sizeof *sfx);
+  sfx->b[0] = (uint8_t)(len_in_bytes >> 8);
+  sfx->b[1] = (uint8_t)len_in_bytes;
+  uint32_t dl = (uint32_t)dst_len;
+  if (dst_len > 255) {
+    DevState& d = ctx->devs[0];
+    Lane& L = d.lane[0];
+    dl = 56;
+    CU_TRY(ctx, cudaSetDevice(d.dev));
+    ST_TRY(ensure(ctx, L, B_AUX, dst_len + 64));
+    uint8_t* buf = (uint8_t*)L.buf[B_AUX];
+    CU_TRY(ctx, cudaMemcpyAsync(buf, dst, dst_len, cudaMemcpyHostToDevice, L.s()));
+    xof_oversize_dst_kernel<<<1, 1, 0, L.s()>>>(buf, dst_len, buf + dst_len);
+    LAUNCHED(ctx);
+    CU_TRY(ctx, cudaMemcpyAsync(sfx->b + 2, buf + dst_len, 56, cudaMemcpyDeviceToHost, L.s()));
+    CU_TRY(ctx, cudaStreamSynchronize(L.s()));
+  } else {
+    memcpy(sfx->b + 2, dst, dst_len);
+  }
+  sfx->b[2 + dl] = (uint8_t)dl;
+  sfx->len = dl + 3;
+  return ECG_OK;
+}
+// hash to group (mode 0: RO, 1: NU) or hash to scalar (mode 2) over a batch of messages (msgs + n + 1 offsets)
+static ecg_status decaf448_hash_entry(ecg_ctx* ctx, const char* who, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
+                                      size_t dst_len, int mode, uint8_t* out56) {
+  if (!ctx) return ECG_EINVAL;
+  if (!dst || dst_len == 0) {  // ExpandMsgXofError::EmptyDst, at any n
+    ctx->err = std::string(who) + ": a non-empty domain separation tag is required";
+    return ECG_EINVAL;
+  }
+  if (n == 0) return ECG_OK;
+  if (!offsets || !out56) {
+    ctx->err = std::string(who) + ": null pointer";
+    return ECG_EINVAL;
+  }
+  ecg_status st = ed448_check_offsets(ctx, who, n, offsets, msgs);
+  if (st != ECG_OK) return st;
+  XofSuffix sfx;
+  if ((st = decaf448_suffix(ctx, dst, dst_len, mode == 0 ? 112 : mode == 1 ? 56 : 64, &sfx)) != ECG_OK) return st;
+  st = run_chunked(ctx, n, (mode == 2 ? DECAF448_H2S_MINBLK : DECAF448_H2C_MINBLK) * DECAF448_BLOCK, [](DevState&) { return ECG_OK; },
+                   [&](DevState&, Lane& L, size_t off, size_t cnt) {
+                     DevPtrs dp;
+                     ST_TRY(begin_lane(ctx, L));
+                     const uint8_t* dmsgs;
+                     const uint64_t* doffs;
+                     uint64_t base;
+                     ST_TRY(stage_msgs(ctx, L, B_A, B_X, msgs, offsets, off, cnt, &dmsgs, &doffs, &base));
+                     ST_TRY(stage_out(ctx, L, off, cnt, out56, 56, nullptr, dp));
+                     const unsigned g = grid_for(cnt, DECAF448_BLOCK);
+                     DOM_BEGIN(ctx, L);
+                     if (mode == 0)
+                       decaf448_h2c_kernel<FpEd448, false><<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                     else if (mode == 1)
+                       decaf448_h2c_kernel<FpEd448, true><<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                     else
+                       decaf448_h2s_kernel<<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                     LAUNCHED(ctx);
+                     DOM_END(ctx, L);
+                     return copy_back(ctx, L, off, cnt, out56, 56, nullptr, dp);
+                   });
+  return st == ECG_OK ? st : fail(ctx, st);
+}
+ECG_API(ecg_decaf448_hash_to_curve_batch)(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
+                                          size_t dst_len, int nonuniform, uint8_t* out56) {
+  return decaf448_hash_entry(ctx, "ecg_decaf448_hash_to_curve_batch", n, msgs, offsets, dst, dst_len, nonuniform ? 1 : 0, out56);
+}
+ECG_API(ecg_decaf448_hash_to_scalar_batch)(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
+                                           size_t dst_len, uint8_t* out56) {
+  return decaf448_hash_entry(ctx, "ecg_decaf448_hash_to_scalar_batch", n, msgs, offsets, dst, dst_len, 2, out56);
 }
 #endif

@@ -14,6 +14,10 @@ bench.py.  It mirrors the reference's names for the hot path:
     Engine.ed448_mul(k57, P57)                 EdwardsPoint * EdwardsScalar over a batch (edwards/extended.rs:698-741)
     Engine.ed448_mul_gen(k57)                  EdwardsPoint::mul_by_generator over a batch
     Engine.ed448_lincomb(k57, P57)             LinearCombination::lincomb for EdwardsPoint (extended.rs:310-312)
+    Engine.decaf448_mul / _mul_gen / _lincomb  DecafPoint * DecafScalar, DecafPoint::GENERATOR * k, LinearCombination
+    Engine.decaf448_check(P56)                 CompressedDecaf::decompress verdicts (decaf/points.rs:555-593)
+    Engine.decaf448_hash_to_curve(msgs, dst)   hash_from_bytes / encode_from_bytes for Decaf448 (ExpandMsgXof<Shake256>)
+    Engine.decaf448_hash_to_scalar(msgs, dst)  hash_to_scalar::<Decaf448, ExpandMsgXof<Shake256>, U64>
 
 Buffers are numpy uint8 arrays (host mode) or raw device pointers (device mode, ECG_FLAG_DEVICE_PTRS).
 There is NO CPU fallback: if libecgpu.so is missing, or no CUDA device is present, construction raises.
@@ -59,6 +63,8 @@ EXPORTS = [
     "ecg_batch_normalize_hom", "ecg_mul_batch_x", "ecg_field_sqrt_batch",
     "ecg_hash_to_curve_batch", "ecg_hash_to_scalar_batch", "ecg_sm2dsa_verify_batch", "ecg_ecdsa_recover_batch",
     "ecg_x448_batch", "ecg_ed448_verify_batch", "ecg_ed448_mul_batch", "ecg_ed448_mul_gen_batch", "ecg_ed448_lincomb",
+    "ecg_decaf448_mul_batch", "ecg_decaf448_mul_gen_batch", "ecg_decaf448_lincomb", "ecg_decaf448_check_batch",
+    "ecg_decaf448_hash_to_curve_batch", "ecg_decaf448_hash_to_scalar_batch",
 ]
 
 
@@ -154,6 +160,14 @@ def load_library(path: Optional[str] = None) -> ctypes.CDLL:
     lib.ecg_ed448_mul_gen_batch.restype = ctypes.c_int
     lib.ecg_ed448_lincomb.argtypes = [vp, sz, u8p, u8p, u8p]
     lib.ecg_ed448_lincomb.restype = ctypes.c_int
+    lib.ecg_decaf448_mul_batch.argtypes = [vp, sz, u8p, u8p, u8p]
+    lib.ecg_decaf448_mul_gen_batch.argtypes = [vp, sz, u8p, u8p]
+    lib.ecg_decaf448_lincomb.argtypes = [vp, sz, u8p, u8p, u8p]
+    lib.ecg_decaf448_check_batch.argtypes = [vp, sz, u8p, u8p]
+    lib.ecg_decaf448_hash_to_curve_batch.argtypes = [vp, sz, u8p, u8p, u8p, sz, ctypes.c_int, u8p]
+    lib.ecg_decaf448_hash_to_scalar_batch.argtypes = [vp, sz, u8p, u8p, u8p, sz, u8p]
+    for f in ("mul_batch", "mul_gen_batch", "lincomb", "check_batch", "hash_to_curve_batch", "hash_to_scalar_batch"):
+        getattr(lib, "ecg_decaf448_" + f).restype = ctypes.c_int
     lib.ecg_version.argtypes = []
     lib.ecg_version.restype = ctypes.c_char_p
     if path is None:
@@ -590,6 +604,71 @@ class Engine:
         self._check(self.lib.ecg_ed448_lincomb(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out)))
         return out
 
+    def decaf448_mul(self, k56, P56, out=None):
+        """Decaf448: out[i] = [k[i]] P[i] (n x 56 encodings; DecafPoint * DecafScalar).  Scalars are 56-byte little-endian,
+        accepted iff DecafScalar::from_canonical_bytes accepts them (ScalarRangeError with the smallest index otherwise);
+        points are accepted iff CompressedDecaf::decompress accepts them (NotOnCurveError otherwise)."""
+        n = np.asarray(k56).size // 56
+        k56 = _u8(k56, 56 * n, "k56")
+        P56 = _u8(P56, 56 * n, "P56")
+        out = _out(out, 56 * n, "out")
+        self._check(self.lib.ecg_decaf448_mul_batch(self._ctx, n, _ptr(k56), _ptr(P56), _ptr(out)))
+        return out.reshape(n, 56)
+
+    def decaf448_mul_gen(self, k56, out=None):
+        """Decaf448: out[i] = [k[i]] G (DecafPoint::GENERATOR), n x 56 encodings"""
+        n = np.asarray(k56).size // 56
+        k56 = _u8(k56, 56 * n, "k56")
+        out = _out(out, 56 * n, "out")
+        self._check(self.lib.ecg_decaf448_mul_gen_batch(self._ctx, n, _ptr(k56), _ptr(out)))
+        return out.reshape(n, 56)
+
+    def decaf448_lincomb(self, k56, P56):
+        """Decaf448: sum_i [k[i]] P[i] as one 56-byte encoding (n = 0: the identity, 56 zero bytes)"""
+        n = np.asarray(k56).size // 56
+        k56 = _u8(k56, 56 * n, "k56")
+        P56 = _u8(P56, 56 * n, "P56")
+        out = np.empty(56, np.uint8)
+        self._check(self.lib.ecg_decaf448_lincomb(self._ctx, n, _ptr(k56), _ptr(P56), _ptr(out)))
+        return out
+
+    def decaf448_check(self, P56, ok=None):
+        """Decaf448: ok[i] = 1 iff CompressedDecaf::decompress accepts P[i] (verdicts, never an error)"""
+        n = np.asarray(P56).size // 56
+        P56 = _u8(P56, 56 * n, "P56")
+        ok = _out(ok, n, "ok")
+        self._check(self.lib.ecg_decaf448_check_batch(self._ctx, n, _ptr(P56), _ptr(ok)))
+        return ok
+
+    def decaf448_hash_to_curve(self, msgs, dst: bytes, nonuniform: bool = False):
+        """Decaf448 hash_from_bytes (RO) / encode_from_bytes (NU) with ExpandMsgXof<Shake256> -> n x 56 encodings"""
+        data, offs = self._pack_messages(msgs)
+        return self.decaf448_hash_to_curve_packed(data, offs, dst, nonuniform)
+
+    def decaf448_hash_to_curve_packed(self, data, offsets, dst: bytes, nonuniform: bool = False, out=None):
+        """the same over messages already laid out as the C ABI takes them (data + n + 1 uint64 offsets)"""
+        offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = offs.size - 1
+        if n < 0 or int(offs[-1]) > np.asarray(data).size:
+            raise ValueError("offsets: n + 1 ascending byte offsets into data")
+        data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+        if data.size == 0:
+            data = np.zeros(1, np.uint8)
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        out = _out(out, 56 * n, "out")
+        self._check(self.lib.ecg_decaf448_hash_to_curve_batch(self._ctx, n, _ptr(data), _ptr(offs), _ptr(d), len(dst), 1 if nonuniform else 0,
+                                                              _ptr(out)))
+        return out.reshape(n, 56)
+
+    def decaf448_hash_to_scalar(self, msgs, dst: bytes):
+        """hash_to_scalar::<Decaf448, ExpandMsgXof<Shake256>, U64> over a batch -> n x 56 little-endian scalars"""
+        n = len(msgs)
+        data, offs = self._pack_messages(msgs)
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        out = np.empty(56 * n, np.uint8)
+        self._check(self.lib.ecg_decaf448_hash_to_scalar_batch(self._ctx, n, _ptr(data), _ptr(offs), _ptr(d), len(dst), _ptr(out)))
+        return out.reshape(n, 56)
+
     # ---- raw-pointer API (device_ptrs=True): all arguments are integer CUDA device addresses ----
     def mul_batch_ptr(self, curve, n, k, P_xy, P_inf, out_xy, out_inf):
         self._check(self.lib.ecg_mul_batch(self._ctx, CURVE_IDS[curve], n, _ptr(k), _ptr(P_xy), _ptr(P_inf), _ptr(out_xy), _ptr(out_inf)))
@@ -640,6 +719,33 @@ class Engine:
     def ed448_lincomb_ptr(self, n, k57, P57, out57):
         """ecg_ed448_lincomb on device buffers (out57: 57 bytes)"""
         self._check(self.lib.ecg_ed448_lincomb(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out57)))
+
+    def decaf448_mul_ptr(self, n, k56, P56, out56):
+        """ecg_decaf448_mul_batch on device buffers (56-byte records, 4-byte aligned)"""
+        self._check(self.lib.ecg_decaf448_mul_batch(self._ctx, n, _ptr(k56), _ptr(P56), _ptr(out56)))
+
+    def decaf448_mul_gen_ptr(self, n, k56, out56):
+        """ecg_decaf448_mul_gen_batch on device buffers"""
+        self._check(self.lib.ecg_decaf448_mul_gen_batch(self._ctx, n, _ptr(k56), _ptr(out56)))
+
+    def decaf448_lincomb_ptr(self, n, k56, P56, out56):
+        """ecg_decaf448_lincomb on device buffers (out56: 56 bytes)"""
+        self._check(self.lib.ecg_decaf448_lincomb(self._ctx, n, _ptr(k56), _ptr(P56), _ptr(out56)))
+
+    def decaf448_check_ptr(self, n, P56, ok):
+        """ecg_decaf448_check_batch on device buffers"""
+        self._check(self.lib.ecg_decaf448_check_batch(self._ctx, n, _ptr(P56), _ptr(ok)))
+
+    def decaf448_hash_to_curve_ptr(self, n, msgs, offsets, out56, dst: bytes, nonuniform: bool = False):
+        """ecg_decaf448_hash_to_curve_batch on device buffers (offsets: n + 1 uint64, 8-byte aligned); the DST is host bytes"""
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        self._check(self.lib.ecg_decaf448_hash_to_curve_batch(self._ctx, n, _ptr(msgs), _ptr(offsets), _ptr(d), len(dst), 1 if nonuniform else 0,
+                                                              _ptr(out56)))
+
+    def decaf448_hash_to_scalar_ptr(self, n, msgs, offsets, out56, dst: bytes):
+        """ecg_decaf448_hash_to_scalar_batch on device buffers; the DST is host bytes"""
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        self._check(self.lib.ecg_decaf448_hash_to_scalar_batch(self._ctx, n, _ptr(msgs), _ptr(offsets), _ptr(d), len(dst), _ptr(out56)))
 
     def timing_enable(self, on: bool = True):
         self._check(self.lib.ecg_timing_enable(self._ctx, 1 if on else 0))

@@ -15,6 +15,9 @@
 //   Engine::ed448_verify(pk, sig, msgs, ctx, ph)      <->  ed448 VerifyingKey::verify_raw / verify_ctx / verify_prehashed
 //   Engine::ed448_mul / ed448_mul_gen / ed448_lincomb <->  EdwardsPoint * EdwardsScalar, Group::mul_by_generator,
 //                                                         LinearCombination::lincomb (ed448-goldilocks/src/edwards/extended.rs)
+//   Engine::decaf448_mul / decaf448_mul_gen / decaf448_lincomb / decaf448_check / decaf448_hash_to_curve /
+//   decaf448_hash_to_scalar                          <->  DecafPoint * DecafScalar, GENERATOR * k, LinearCombination,
+//                                                         CompressedDecaf::decompress, GroupDigest / hash_to_scalar for Decaf448
 // The typed surface below is for the 256-bit curves with big-endian records (secp256k1, P-256, sm2, brainpoolP256r1/t1);
 // the other curves of include/ecgpu.h (48 / 28 / 24-byte records, bign's little-endian records) are reached through the
 // C ABI directly or the Python mirror, which sizes its buffers per curve.
@@ -199,6 +202,55 @@ class Engine {
     return out;
   }
 
+  // ---- Decaf448 (RFC 9496), 56-byte scalars and encodings; the same on an Engine of any curve ----
+  using Decaf448Bytes = std::array<uint8_t, 56>;
+  // out[i] = [k[i]] P[i]: DecafPoint * DecafScalar
+  std::vector<Decaf448Bytes> decaf448_mul(const std::vector<Decaf448Bytes>& k, const std::vector<Decaf448Bytes>& P) {
+    check_sizes(k.size(), P.size());
+    std::vector<Decaf448Bytes> out(k.size());
+    check(ecg_decaf448_mul_batch(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<const uint8_t*>(P.data()),
+                                 reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+  // out[i] = [k[i]] G (DecafPoint::GENERATOR)
+  std::vector<Decaf448Bytes> decaf448_mul_gen(const std::vector<Decaf448Bytes>& k) {
+    std::vector<Decaf448Bytes> out(k.size());
+    check(ecg_decaf448_mul_gen_batch(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+  // sum [k[i]] P[i] (empty input: the identity, 56 zero bytes)
+  Decaf448Bytes decaf448_lincomb(const std::vector<Decaf448Bytes>& k, const std::vector<Decaf448Bytes>& P) {
+    check_sizes(k.size(), P.size());
+    Decaf448Bytes out{};
+    check(ecg_decaf448_lincomb(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<const uint8_t*>(P.data()), out.data()));
+    return out;
+  }
+  // result[i] = true iff CompressedDecaf::decompress accepts P[i]
+  std::vector<bool> decaf448_check(const std::vector<Decaf448Bytes>& P) {
+    std::vector<uint8_t> ok(P.size());
+    check(ecg_decaf448_check_batch(ctx_, P.size(), reinterpret_cast<const uint8_t*>(P.data()), ok.data()));
+    return std::vector<bool>(ok.begin(), ok.end());
+  }
+  // hash_from_bytes (nonuniform = false) / encode_from_bytes for decaf448_XOF:SHAKE256_D448MAP_{RO,NU}_ under one DST
+  std::vector<Decaf448Bytes> decaf448_hash_to_curve(const std::vector<std::vector<uint8_t>>& msgs, const std::vector<uint8_t>& dst,
+                                                    bool nonuniform = false) {
+    std::vector<uint64_t> offsets;
+    std::vector<uint8_t> data = pack(msgs, offsets);
+    std::vector<Decaf448Bytes> out(msgs.size());
+    check(ecg_decaf448_hash_to_curve_batch(ctx_, msgs.size(), data.empty() ? nullptr : data.data(), offsets.data(), dst.data(), dst.size(),
+                                           nonuniform ? 1 : 0, reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+  // hash_to_scalar::<Decaf448, ExpandMsgXof<Shake256>, U64>: 56-byte little-endian scalars
+  std::vector<Decaf448Bytes> decaf448_hash_to_scalar(const std::vector<std::vector<uint8_t>>& msgs, const std::vector<uint8_t>& dst) {
+    std::vector<uint64_t> offsets;
+    std::vector<uint8_t> data = pack(msgs, offsets);
+    std::vector<Decaf448Bytes> out(msgs.size());
+    check(ecg_decaf448_hash_to_scalar_batch(ctx_, msgs.size(), data.empty() ? nullptr : data.data(), offsets.data(), dst.data(), dst.size(),
+                                            reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+
   // ---- widening (SURVEY 8(f)): verification, wire format, key agreement ----
   using Bytes32 = std::array<uint8_t, 32>;
   using Sig64 = std::array<uint8_t, 64>;
@@ -332,6 +384,16 @@ class Engine {
     return a;
   }
   static const uint8_t* flat(const std::vector<Scalar>& s) { return reinterpret_cast<const uint8_t*>(s.data()); }
+  // messages back to back and their n + 1 offsets (the layout of the message-taking entries)
+  static std::vector<uint8_t> pack(const std::vector<std::vector<uint8_t>>& msgs, std::vector<uint64_t>& offsets) {
+    std::vector<uint8_t> data;
+    offsets.assign(msgs.size() + 1, 0);
+    for (size_t i = 0; i < msgs.size(); i++) {
+      data.insert(data.end(), msgs[i].begin(), msgs[i].end());
+      offsets[i + 1] = data.size();
+    }
+    return data;
+  }
   void pack(const std::vector<AffinePoint>& pts) {
     xy_.resize(64 * pts.size());
     inf_.resize(pts.size());

@@ -105,7 +105,8 @@ typedef enum {
                                    ecg_ed448_lincomb) follow the same rule: a masked scan of the 8-entry table, a masked
                                    negation and a masked "add ell when k is even", k*B through the variable-base routine on
                                    B.  The Edwards formulas are complete, so that path has no scalar-dependent branch at
-                                   all. */
+                                   all.  The Decaf448 entries do the same (k*G on the decoded generator), and their
+                                   encoding is branch-free. */
 
 /* Create a context on the given CUDA devices (NULL/0 = device 0).  With several devices a host-pointer
  * batch is split into contiguous index ranges, one per device (SURVEY.md §8(e)); there is no
@@ -338,6 +339,46 @@ ecg_status ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, u
  * extended.rs:310-312, the reference's default sum of products), one 57-byte record; n = 0 writes the identity. */
 ecg_status ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t out57[57]);
 
+/* ---- Decaf448 (RFC 9496): the prime-order group of ed448-goldilocks (DecafPoint, CompressedDecaf, DecafScalar) --------
+ * Records: a scalar is 56 bytes little-endian (DecafScalarBytes), accepted iff DecafScalar::from_canonical_bytes
+ * accepts it (ed448-goldilocks/src/decaf/scalar.rs:22-32): byte 55 >> 6 == 0 and the value is < ell, else
+ * ECG_ESCALAR_RANGE.  A point is 56 bytes s, accepted iff CompressedDecaf::decompress accepts it (decaf/points.rs:
+ * 555-593): s < p, s even, and the inverse square root exists; 56 zero bytes are the identity; else ECG_ENOT_ON_CURVE.
+ * An output is DecafPoint::compress (decaf/points.rs:49-67); the identity is 56 zero bytes.
+ * A refused record fails the whole call; ecg_last_error_index gives the smallest offending index.
+ * Errors: ECG_EINVAL (null ctx; a null array with n > 0; for lincomb a null out56 at any n) and CUDA errors.
+ * With ECG_FLAG_DEVICE_PTRS every array is a device pointer; the 56-byte records are 4-byte aligned (as X448's, else
+ * ECG_EINVAL), messages and ok bytes may sit anywhere, offsets are 8-byte aligned.  ECG_FLAG_ZEROIZE scrubs the staged records, the per-thread tables and the intermediate points on the
+ * device.  ECG_FLAG_CONSTTIME: as for the Ed448 group entries (k*G through the variable-base routine on the decoded
+ * generator); outputs are identical either way.  A multi-device ctx splits the batch into contiguous index ranges. */
+
+/* out56[i] = [k56[i]] P56[i]: Mul<&DecafScalar> for DecafPoint over a batch; n = 0 is ECG_OK. */
+ecg_status ecg_decaf448_mul_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* P56, uint8_t* out56);
+
+/* out56[i] = [k56[i]] G (DecafPoint::GENERATOR) over a batch: the encoding of [(-2 k) mod ell] B from the Ed448
+ * fixed-base table (built on each device at its first use, shared with ecg_ed448_mul_gen_batch); n = 0 is ECG_OK. */
+ecg_status ecg_decaf448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k56, uint8_t* out56);
+
+/* out56 = sum_i [k56[i]] P56[i]: LinearCombination for DecafPoint, one 56-byte record; n = 0 writes the identity. */
+ecg_status ecg_decaf448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k56, const uint8_t* P56, uint8_t out56[56]);
+
+/* ok[i] = 1 iff CompressedDecaf::decompress accepts P56[i], else 0: per-record verdicts, never a refusal error (what a
+ * server needs to filter client elements without failing a batch); n = 0 is ECG_OK. */
+ecg_status ecg_decaf448_check_batch(ecg_ctx* ctx, size_t n, const uint8_t* P56, uint8_t* ok);
+
+/* Hash to group for decaf448_XOF:SHAKE256_D448MAP_RO_ / _NU_ (GroupDigest for Decaf448, ed448-goldilocks/src/lib.rs:
+ * 159-164): message i = msgs[offsets[i] .. offsets[i+1]) (as in ecg_hash_to_curve_batch), one DST for the call (host
+ * pointer; empty: ECG_EINVAL; over 255 bytes: replaced by SHAKE256("H2C-OVERSIZE-DST-" || DST, 56)).
+ * nonuniform = 0: hash_from_bytes (expand_message_xof to 112 bytes, each 56-byte half little-endian mod p through
+ * map_to_curve_decaf448, the two points added); != 0: encode_from_bytes (56 bytes, one map).  out56[i] = the encoding. */
+ecg_status ecg_decaf448_hash_to_curve_batch(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets,
+                                            const uint8_t* dst, size_t dst_len, int nonuniform, uint8_t* out56);
+
+/* out56[i] = hash_to_scalar::<Decaf448, ExpandMsgXof<Shake256>, U64>: 64 expanded bytes read little-endian, reduced mod
+ * ell, as DecafScalar::to_repr (56 bytes little-endian); messages and DST as above. */
+ecg_status ecg_decaf448_hash_to_scalar_batch(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets,
+                                             const uint8_t* dst, size_t dst_len, uint8_t* out56);
+
 /* ---- measurement helpers (not part of the reference-facing surface) ---- */
 
 /* Integer-pipe microbenchmark on device 0 of the ctx: which = 0 IMAD.WIDE.U32.X carry chains (the
@@ -347,7 +388,8 @@ ecg_status ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const u
 ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double* ops_per_s, double* elapsed_ms);
 
 /* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication, the X448 ladder,
- * the Ed448 verification kernel, the Ed448 scalar-multiplication kernels)
+ * the Ed448 verification kernel, the Ed448 and Decaf448 scalar-multiplication kernels, the Decaf448 check and hash
+ * kernels)
  * with CUDA events on the launching stream; ecg_timing_read returns the accumulated device milliseconds
  * (max over the ctx's devices per call) and the number of calls since ecg_timing_enable. */
 ecg_status ecg_timing_enable(ecg_ctx* ctx, int on);

@@ -101,6 +101,22 @@ unsafe extern "C" {
     pub fn ecg_ed448_mul_gen_batch(ctx: *mut ecg_ctx, n: usize, k57: *const u8, out57: *mut u8) -> i32;
     /// Ed448 group: `out57 = EdwardsPoint::lincomb(&[(P57[i], k57[i])])` (extended.rs:310-312); n = 0: the identity
     pub fn ecg_ed448_lincomb(ctx: *mut ecg_ctx, n: usize, k57: *const u8, p57: *const u8, out57: *mut u8) -> i32;
+    /// Decaf448: `out56[i] = k56[i] * P56[i]` (`Mul<&DecafScalar> for DecafPoint`); 56-byte scalars
+    /// (`DecafScalar::from_canonical_bytes`) and encodings (`CompressedDecaf::decompress`)
+    pub fn ecg_decaf448_mul_batch(ctx: *mut ecg_ctx, n: usize, k56: *const u8, p56: *const u8, out56: *mut u8) -> i32;
+    /// Decaf448: `out56[i] = DecafPoint::GENERATOR * k56[i]`
+    pub fn ecg_decaf448_mul_gen_batch(ctx: *mut ecg_ctx, n: usize, k56: *const u8, out56: *mut u8) -> i32;
+    /// Decaf448: `out56 = sum k56[i] * P56[i]` (`LinearCombination`); n = 0: the identity (56 zero bytes)
+    pub fn ecg_decaf448_lincomb(ctx: *mut ecg_ctx, n: usize, k56: *const u8, p56: *const u8, out56: *mut u8) -> i32;
+    /// Decaf448: `ok[i] = CompressedDecaf(P56[i]).decompress().is_some()`
+    pub fn ecg_decaf448_check_batch(ctx: *mut ecg_ctx, n: usize, p56: *const u8, ok: *mut u8) -> i32;
+    /// Decaf448 `hash_from_bytes` (nonuniform = 0) / `encode_from_bytes` with `ExpandMsgXof<Shake256>`; message i =
+    /// `msgs[offsets[i]..offsets[i + 1]]`, one DST
+    pub fn ecg_decaf448_hash_to_curve_batch(ctx: *mut ecg_ctx, n: usize, msgs: *const u8, offsets: *const u64, dst: *const u8,
+                                            dst_len: usize, nonuniform: i32, out56: *mut u8) -> i32;
+    /// `hash_to_scalar::<Decaf448, ExpandMsgXof<Shake256>, U64>` over a batch (56-byte little-endian scalars)
+    pub fn ecg_decaf448_hash_to_scalar_batch(ctx: *mut ecg_ctx, n: usize, msgs: *const u8, offsets: *const u64, dst: *const u8,
+                                             dst_len: usize, out56: *mut u8) -> i32;
     pub fn ecg_kernel_launches(ctx: *const ecg_ctx) -> u64;
 }
 
@@ -206,6 +222,67 @@ impl GpuEngine {
         let mut out = [0u8; 57];
         // SAFETY: k and p hold k.len() records of 57 bytes, out 57 bytes.
         let rc = unsafe { ecg_ed448_lincomb(self.ctx, k.len(), k.as_ptr().cast(), p.as_ptr().cast(), out.as_mut_ptr()) };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Decaf448, for an engine of any curve: `out[i] = k[i] * P[i]` (`DecafPoint * DecafScalar`); a scalar
+    /// `DecafScalar::from_canonical_bytes` refuses or an encoding `CompressedDecaf::decompress` refuses fails the call
+    /// with its smallest index.
+    pub fn batch_mul_decaf448(&mut self, k: &[[u8; 56]], p: &[[u8; 56]]) -> Result<Vec<[u8; 56]>, GpuError> {
+        assert_eq!(k.len(), p.len());
+        let mut out = vec![[0u8; 56]; k.len()];
+        // SAFETY: k, p and out hold k.len() records of 56 bytes.
+        let rc = unsafe { ecg_decaf448_mul_batch(self.ctx, k.len(), k.as_ptr().cast(), p.as_ptr().cast(), out.as_mut_ptr().cast()) };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Decaf448: `out[i] = DecafPoint::GENERATOR * k[i]`
+    pub fn batch_mul_gen_decaf448(&mut self, k: &[[u8; 56]]) -> Result<Vec<[u8; 56]>, GpuError> {
+        let mut out = vec![[0u8; 56]; k.len()];
+        // SAFETY: k and out hold k.len() records of 56 bytes.
+        let rc = unsafe { ecg_decaf448_mul_gen_batch(self.ctx, k.len(), k.as_ptr().cast(), out.as_mut_ptr().cast()) };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Decaf448: `sum k[i] * P[i]`; empty input gives the identity
+    pub fn lincomb_decaf448(&mut self, k: &[[u8; 56]], p: &[[u8; 56]]) -> Result<[u8; 56], GpuError> {
+        assert_eq!(k.len(), p.len());
+        let mut out = [0u8; 56];
+        // SAFETY: k and p hold k.len() records of 56 bytes, out 56 bytes.
+        let rc = unsafe { ecg_decaf448_lincomb(self.ctx, k.len(), k.as_ptr().cast(), p.as_ptr().cast(), out.as_mut_ptr()) };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Decaf448: whether `CompressedDecaf(p[i]).decompress()` succeeds, per record (never an error for a bad record)
+    pub fn batch_check_decaf448(&mut self, p: &[[u8; 56]]) -> Result<Vec<bool>, GpuError> {
+        let mut ok = vec![0u8; p.len()];
+        // SAFETY: p holds p.len() records of 56 bytes, ok p.len() bytes.
+        let rc = unsafe { ecg_decaf448_check_batch(self.ctx, p.len(), p.as_ptr().cast(), ok.as_mut_ptr()) };
+        self.check(rc).map(|_| ok.into_iter().map(|b| b != 0).collect())
+    }
+
+    /// Decaf448 hash to group (`hash_from_bytes`, or `encode_from_bytes` with `nonuniform`) or, with `scalar`,
+    /// `hash_to_scalar` under one DST: one 56-byte record per message
+    pub fn batch_hash_decaf448(&mut self, msgs: &[&[u8]], dst: &[u8], nonuniform: bool, scalar: bool) -> Result<Vec<[u8; 56]>, GpuError> {
+        let n = msgs.len();
+        let mut offsets = Vec::with_capacity(n + 1);
+        let mut data = Vec::new();
+        offsets.push(0u64);
+        for m in msgs {
+            data.extend_from_slice(m);
+            offsets.push(data.len() as u64);
+        }
+        let mut out = vec![[0u8; 56]; n];
+        let data_ptr = if data.is_empty() { core::ptr::null() } else { data.as_ptr() };
+        // SAFETY: offsets holds n + 1 entries into data, dst dst.len() bytes, out n records of 56 bytes.
+        let rc = unsafe {
+            if scalar {
+                ecg_decaf448_hash_to_scalar_batch(self.ctx, n, data_ptr, offsets.as_ptr(), dst.as_ptr(), dst.len(), out.as_mut_ptr().cast())
+            } else {
+                ecg_decaf448_hash_to_curve_batch(self.ctx, n, data_ptr, offsets.as_ptr(), dst.as_ptr(), dst.len(), nonuniform as i32,
+                                                 out.as_mut_ptr().cast())
+            }
+        };
         self.check(rc).map(|_| out)
     }
 

@@ -95,6 +95,22 @@ def main():
     assert bytes(m[0]) == ed448_group_model.mul(ed448_group_model.enc_scalar(kg[0]), pk57), "ed448 mul"
     lc = eng.ed448_lincomb(K448, P448)
     assert bytes(lc) == ed448_group_model.lincomb([ed448_group_model.enc_scalar(k) for k in kg], [pk57] * 5), "ed448 lincomb"
+    # Decaf448: one small call per entry, against the model
+    import decaf448_model
+    K56 = np.frombuffer(b"".join(decaf448_model.enc_scalar(k) for k in kg), np.uint8)
+    dg = [bytes(r) for r in eng.decaf448_mul_gen(K56)]
+    assert dg == [decaf448_model.mul_gen(decaf448_model.enc_scalar(k)) for k in kg], "decaf448 mul_gen"
+    P56 = np.frombuffer(b"".join(dg), np.uint8)
+    dm = eng.decaf448_mul(K56, P56)
+    assert bytes(dm[0]) == decaf448_model.mul(decaf448_model.enc_scalar(kg[0]), dg[0]), "decaf448 mul"
+    dl = eng.decaf448_lincomb(K56, P56)
+    assert bytes(dl) == decaf448_model.lincomb([decaf448_model.enc_scalar(k) for k in kg], dg), "decaf448 lincomb"
+    assert list(eng.decaf448_check(np.frombuffer(dg[0] + bytes([1]) * 56, np.uint8))) == [1, 0], "decaf448 check"
+    dst = decaf448_model.HASH_TO_CURVE_ID
+    assert [bytes(r) for r in eng.decaf448_hash_to_curve(m448, dst)] == [decaf448_model.hash_to_curve(m, dst) for m in m448], "decaf448 h2c"
+    assert [bytes(r) for r in eng.decaf448_hash_to_curve(m448, bytes(300), True)] == [decaf448_model.hash_to_curve(m, bytes(300), True)
+                                                                                      for m in m448], "decaf448 h2c nu"
+    assert [bytes(r) for r in eng.decaf448_hash_to_scalar(m448, dst)] == [decaf448_model.hash_to_scalar(m, dst) for m in m448], "decaf448 h2s"
     eng.close()
     print("sanitize workload OK")
 
