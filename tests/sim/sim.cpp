@@ -75,6 +75,27 @@ static void sim_launch(size_t threads, unsigned block, Body body) {
       body();
     }
 }
+// the same, the blocks shared out over the host's cores: for kernels without __shared__ whose threads write disjoint
+// memory or update it atomically (the bucket and reduction kernels over the 2^17-slot windows of the widest geometry)
+template <class Body>
+static void sim_launch_par(size_t threads, unsigned block, Body body) {
+  unsigned grid = (unsigned)((threads + block - 1) / block);
+  if (grid == 0) grid = 1;
+  unsigned nt = std::max(1u, std::min(grid, std::thread::hardware_concurrency()));
+  std::vector<std::thread> th;
+  for (unsigned i = 0; i < nt; i++)
+    th.emplace_back([=, &body] {
+      gridDim.x = grid;
+      blockDim.x = block;
+      for (unsigned b = i; b < grid; b += nt)
+        for (unsigned t = 0; t < block; t++) {
+          blockIdx.x = b;
+          threadIdx.x = t;
+          body();
+        }
+    });
+  for (auto& x : th) x.join();
+}
 // `grid` blocks of `block` real threads each (kernels that use __shared__ / __syncthreads), one block at a time
 template <class Body>
 static void sim_launch_blocks(unsigned grid, unsigned block, Body body) {
@@ -508,6 +529,16 @@ int sim_msm_recode(const uint8_t* m_le36, int c, int nbits, int32_t* out) {
   msm_recode(out, m, g);
   return g.W;
 }
+// the same on nm little-endian 32-bit limbs (the prep kernel passes NL + 1: 13 for the 384-bit curves, 18 for P-521)
+int sim_msm_recode_n(const uint32_t* m, int nm, int c, int nbits, int32_t* out) {
+  MsmGeom g;
+  g.c = c;
+  g.nbits = nbits;
+  g.W = (nbits + c - 1) / c;
+  g.nbw = (1u << (c + 1)) + 2;
+  msm_recode(out, m, g, nm);
+  return g.W;
+}
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------------
@@ -670,6 +701,15 @@ static MsmGeom simk_msm_geometry(int curve, size_t n) {  // = msm_geometry (ecgp
   g.nbw = ((uint32_t)1 << (g.c + 1)) + 2;
   return g;
 }
+// out = {c, W, nbits, nbw} of simk_msm_geometry
+extern "C" int sim_msm_geometry(int curve, size_t n, int* out) {
+  MsmGeom g = simk_msm_geometry(curve, n);
+  out[0] = g.c;
+  out[1] = g.W;
+  out[2] = g.nbits;
+  out[3] = (int)g.nbw;
+  return 0;
+}
 
 template <class C>
 static std::vector<uint32_t> simk_reduce_points(std::vector<uint32_t> a, size_t n) {  // = reduce_points
@@ -734,7 +774,7 @@ static bool simk_msm_run(const uint8_t* k, const uint8_t* pxy, const uint8_t* pi
         fprintf(stderr, "msm_order_*: bucket order is not a permutation (bucket %zu seen %u times)\n", b, seen[b]);
         abort();
       }
-    sim_launch(nb, 128, [&] { msm_bucket_kernel<C>(pts.data(), list.data(), offset.data(), nb, bkt.data(), sk, order.data()); });
+    sim_launch_par(nb, 128, [&] { msm_bucket_kernel<C>(pts.data(), list.data(), offset.data(), nb, bkt.data(), sk, order.data()); });
   }
   if (status[0] & MSM_SKEW_FLAG) {  // as finish() + the caller in ecgpu.cu: the flag is consumed, the per-term path runs
     status[0] &= ~MSM_SKEW_FLAG;
@@ -751,7 +791,7 @@ static bool simk_msm_run(const uint8_t* k, const uint8_t* pxy, const uint8_t* pi
     size_t len_low = ((size_t)1 << (g.c - 1));
     for (int q = 0; q < l; q++) len_low = (len_low + (q == 0 ? MSM_CH0 : MSM_CHU) - 1) / (q == 0 ? MSM_CH0 : MSM_CHU);
     len_low = std::min(len_low, lens[l]);
-    sim_launch((size_t)g.W * nchs[l], 128, [&] {
+    sim_launch_par((size_t)g.W * nchs[l], 128, [&] {
       msm_wreduce_kernel<C>(in, n_in, stride, off, lens[l], len_low, g.W, nchs[l], l == 0 ? nullptr : X[l - 1].data(), l, S[l].data(), X[l].data());
     });
   }
@@ -763,11 +803,16 @@ static bool simk_msm_run(const uint8_t* k, const uint8_t* pxy, const uint8_t* pi
 
 template <class C, bool GLV, bool IS_K256>
 static void simk_lincomb_t(int curve, size_t n, const uint8_t* k, const uint8_t* pxy, const uint8_t* pinf, size_t msm_min_terms,
-                           uint8_t* out_xy, uint8_t* out_inf, uint32_t* status, int* path, int bucket_k) {
+                           uint8_t* out_xy, uint8_t* out_inf, uint32_t* status, int* path, int bucket_k, int force_c = 0) {
   std::vector<uint32_t> res;
   *path = 0;
   if (n >= msm_min_terms) {
     MsmGeom g = simk_msm_geometry(curve, n);
+    if (force_c) {  // a window width the product would pick only for a larger n
+      g.c = force_c;
+      g.W = (g.nbits + g.c - 1) / g.c;
+      g.nbw = ((uint32_t)1 << (g.c + 1)) + 2;
+    }
     *path = simk_msm_run<C, GLV>(k, pxy, pinf, n, g, status, res, bucket_k) ? 1 : 2;
   }
   if (*path != 1) {  // per-term kernel + tree sum
@@ -784,8 +829,8 @@ static void simk_lincomb_t(int curve, size_t n, const uint8_t* k, const uint8_t*
   simk_normalize<C>(res, 1, out_xy, out_inf);
 }
 
-extern "C" int simk_lincomb_k(int curve, size_t n, const uint8_t* k, const uint8_t* pxy, const uint8_t* pinf, size_t msm_min_terms,
-                              uint8_t* out_xy, uint8_t* out_inf, uint32_t* status, int* path, int bucket_k) {
+extern "C" int simk_lincomb_c(int curve, size_t n, const uint8_t* k, const uint8_t* pxy, const uint8_t* pinf, size_t msm_min_terms,
+                              uint8_t* out_xy, uint8_t* out_inf, uint32_t* status, int* path, int bucket_k, int force_c) {
   status[0] = 0;
   status[1] = 0xFFFFFFFFu;
   if (n == 0) {  // empty sum = identity
@@ -795,14 +840,18 @@ extern "C" int simk_lincomb_k(int curve, size_t n, const uint8_t* k, const uint8
     return 0;
   }
   if (curve == 0)
-    simk_lincomb_t<CurveK256, true, true>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k);
+    simk_lincomb_t<CurveK256, true, true>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k, force_c);
   else if (curve == 1)
-    simk_lincomb_t<CurveP256, false, false>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k);
+    simk_lincomb_t<CurveP256, false, false>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k, force_c);
   else if (curve == 2)
-    simk_lincomb_t<CurveP384, false, false>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k);
+    simk_lincomb_t<CurveP384, false, false>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k, force_c);
   else
-    SIM_FOR_EXT(curve, (simk_lincomb_t<CV, false, false>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k)));
+    SIM_FOR_EXT(curve, (simk_lincomb_t<CV, false, false>(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k, force_c)));
   return 0;
+}
+extern "C" int simk_lincomb_k(int curve, size_t n, const uint8_t* k, const uint8_t* pxy, const uint8_t* pinf, size_t msm_min_terms,
+                              uint8_t* out_xy, uint8_t* out_inf, uint32_t* status, int* path, int bucket_k) {
+  return simk_lincomb_c(curve, n, k, pxy, pinf, msm_min_terms, out_xy, out_inf, status, path, bucket_k, 0);
 }
 extern "C" int simk_lincomb(int curve, size_t n, const uint8_t* k, const uint8_t* pxy, const uint8_t* pinf, size_t msm_min_terms,
                             uint8_t* out_xy, uint8_t* out_inf, uint32_t* status, int* path) {
