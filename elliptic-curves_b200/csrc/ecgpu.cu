@@ -18,8 +18,8 @@
 //   ECG_TU 1: sm2, brainpoolP256r1/t1, bign-curve256v1 (8 limbs)   ECG_TU 2: brainpoolP384r1/t1 (12 limbs)
 //   ECG_TU 3: P-224 (7 limbs), P-192 (6 limbs)                    ECG_TU 4: P-521 (17 limbs, 66-byte records)
 //   ECG_TU 5: X448 (Curve448, 14 limbs, 56-byte records): the host pipeline and the ladder kernel, no Weierstrass code
-//   ECG_TU 6: Ed448 (the Edwards group on the Curve448 field): verification (SHAKE256) and the group operations, and
-//             Decaf448 on the same point layer; the host pipelines and their kernels
+//   ECG_TU 6: Ed448 (the Edwards group on the Curve448 field): verification (SHAKE256), the group operations and hash
+//             to curve, and Decaf448 on the same point layer; the host pipelines and their kernels
 // Groups 5 and 6 take no ecg_curve and export their own extern "C" entries.
 // The groups 1-3 run the generic kernels over the generic Montgomery field policy (ecg_fe_mont.cuh).
 #ifndef ECG_TU
@@ -31,7 +31,7 @@
 #if ECG_TU == 5
 #include "ecg_x448.cuh"
 #else
-#include "ecg_decaf448.cuh"
+#include "ecg_ed448_h2c.cuh"
 #endif
 using namespace ecg;
 // the status flags of ecg_kernels.cuh that finish() reads; every 56-byte string is a valid X448 input, and an Ed448
@@ -2658,24 +2658,34 @@ static ecg_status decaf448_suffix(ecg_ctx* ctx, const uint8_t* dst, size_t dst_l
   sfx->len = dl + 3;
   return ECG_OK;
 }
-// hash to group (mode 0: RO, 1: NU) or hash to scalar (mode 2) over a batch of messages (msgs + n + 1 offsets)
+// what one hash entry computes: Decaf448 hash to group (RO, NU) and hash to scalar (56-byte records), Ed448 hash to curve
+// (RO, NU) and hash to scalar (57-byte records)
+enum HashMode { H_DECAF_RO, H_DECAF_NU, H_DECAF_SCALAR, H_ED448_RO, H_ED448_NU, H_ED448_SCALAR };
+// expand_message_xof's len_in_bytes, the output record size and the hash kernel's blocks per SM, per HashMode
+static const uint32_t HASH_XOF_LEN[] = {112, 56, 64, 168, 84, 84};
+static const size_t HASH_REC[] = {56, 56, 56, 57, 57, 57};
+static const size_t HASH_MINBLK[] = {DECAF448_H2C_MINBLK, DECAF448_H2C_MINBLK, DECAF448_H2S_MINBLK, ED448H_H2C_MINBLK, ED448H_H2C_MINBLK,
+                                     ED448H_H2S_MINBLK};
+// one hash entry over a batch of messages (msgs + n + 1 offsets).  The Ed448 points leave the hash kernel as extended
+// points (B_JAC) and are compressed by the normalisation kernel of the Ed448 group entries.
 static ecg_status decaf448_hash_entry(ecg_ctx* ctx, const char* who, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
-                                      size_t dst_len, int mode, uint8_t* out56) {
+                                      size_t dst_len, HashMode mode, uint8_t* out) {
   if (!ctx) return ECG_EINVAL;
   if (!dst || dst_len == 0) {  // ExpandMsgXofError::EmptyDst, at any n
     ctx->err = std::string(who) + ": a non-empty domain separation tag is required";
     return ECG_EINVAL;
   }
   if (n == 0) return ECG_OK;
-  if (!offsets || !out56) {
+  if (!offsets || !out) {
     ctx->err = std::string(who) + ": null pointer";
     return ECG_EINVAL;
   }
   ecg_status st = ed448_check_offsets(ctx, who, n, offsets, msgs);
   if (st != ECG_OK) return st;
   XofSuffix sfx;
-  if ((st = decaf448_suffix(ctx, dst, dst_len, mode == 0 ? 112 : mode == 1 ? 56 : 64, &sfx)) != ECG_OK) return st;
-  st = run_chunked(ctx, n, (mode == 2 ? DECAF448_H2S_MINBLK : DECAF448_H2C_MINBLK) * DECAF448_BLOCK, [](DevState&) { return ECG_OK; },
+  if ((st = decaf448_suffix(ctx, dst, dst_len, HASH_XOF_LEN[mode], &sfx)) != ECG_OK) return st;
+  const size_t rec = HASH_REC[mode];
+  st = run_chunked(ctx, n, HASH_MINBLK[mode] * DECAF448_BLOCK, [](DevState&) { return ECG_OK; },
                    [&](DevState&, Lane& L, size_t off, size_t cnt) {
                      DevPtrs dp;
                      ST_TRY(begin_lane(ctx, L));
@@ -2683,27 +2693,53 @@ static ecg_status decaf448_hash_entry(ecg_ctx* ctx, const char* who, size_t n, c
                      const uint64_t* doffs;
                      uint64_t base;
                      ST_TRY(stage_msgs(ctx, L, B_A, B_X, msgs, offsets, off, cnt, &dmsgs, &doffs, &base));
-                     ST_TRY(stage_out(ctx, L, off, cnt, out56, 56, nullptr, dp));
+                     if (mode == H_ED448_RO || mode == H_ED448_NU) ST_TRY(ensure(ctx, L, B_JAC, cnt * ED448G_PT));
+                     ST_TRY(stage_out(ctx, L, off, cnt, out, rec, nullptr, dp));
+                     uint32_t* ext = (uint32_t*)L.buf[B_JAC];
                      const unsigned g = grid_for(cnt, DECAF448_BLOCK);
                      DOM_BEGIN(ctx, L);
-                     if (mode == 0)
-                       decaf448_h2c_kernel<FpEd448, false><<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
-                     else if (mode == 1)
-                       decaf448_h2c_kernel<FpEd448, true><<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
-                     else
-                       decaf448_h2s_kernel<<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                     switch (mode) {
+                       case H_DECAF_RO:
+                         decaf448_h2c_kernel<FpEd448, false><<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                         break;
+                       case H_DECAF_NU:
+                         decaf448_h2c_kernel<FpEd448, true><<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                         break;
+                       case H_DECAF_SCALAR:
+                         decaf448_h2s_kernel<<<g, DECAF448_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                         break;
+                       case H_ED448_RO:
+                         ed448h_h2c_kernel<FpEd448, false><<<g, ED448H_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, ext);
+                         break;
+                       case H_ED448_NU:
+                         ed448h_h2c_kernel<FpEd448, true><<<g, ED448H_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, ext);
+                         break;
+                       case H_ED448_SCALAR:
+                         ed448h_h2s_kernel<<<g, ED448H_BLOCK, 0, L.s()>>>(dmsgs, doffs, base, cnt, sfx, dp.out);
+                         break;
+                     }
                      LAUNCHED(ctx);
                      DOM_END(ctx, L);
-                     return copy_back(ctx, L, off, cnt, out56, 56, nullptr, dp);
+                     if (mode == H_ED448_RO || mode == H_ED448_NU) ST_TRY(ed448g_norm<false>(ctx, L, ext, cnt, dp.out));
+                     return copy_back(ctx, L, off, cnt, out, rec, nullptr, dp);
                    });
   return st == ECG_OK ? st : fail(ctx, st);
 }
 ECG_API(ecg_decaf448_hash_to_curve_batch)(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
                                           size_t dst_len, int nonuniform, uint8_t* out56) {
-  return decaf448_hash_entry(ctx, "ecg_decaf448_hash_to_curve_batch", n, msgs, offsets, dst, dst_len, nonuniform ? 1 : 0, out56);
+  return decaf448_hash_entry(ctx, "ecg_decaf448_hash_to_curve_batch", n, msgs, offsets, dst, dst_len, nonuniform ? H_DECAF_NU : H_DECAF_RO, out56);
 }
 ECG_API(ecg_decaf448_hash_to_scalar_batch)(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
                                            size_t dst_len, uint8_t* out56) {
-  return decaf448_hash_entry(ctx, "ecg_decaf448_hash_to_scalar_batch", n, msgs, offsets, dst, dst_len, 2, out56);
+  return decaf448_hash_entry(ctx, "ecg_decaf448_hash_to_scalar_batch", n, msgs, offsets, dst, dst_len, H_DECAF_SCALAR, out56);
+}
+// ---- Ed448 hash to curve (ecg_ed448_h2c.cuh): the hash pipeline above with 57-byte records --------------------------------
+ECG_API(ecg_ed448_hash_to_curve_batch)(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
+                                       size_t dst_len, int nonuniform, uint8_t* out57) {
+  return decaf448_hash_entry(ctx, "ecg_ed448_hash_to_curve_batch", n, msgs, offsets, dst, dst_len, nonuniform ? H_ED448_NU : H_ED448_RO, out57);
+}
+ECG_API(ecg_ed448_hash_to_scalar_batch)(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets, const uint8_t* dst,
+                                        size_t dst_len, uint8_t* out57) {
+  return decaf448_hash_entry(ctx, "ecg_ed448_hash_to_scalar_batch", n, msgs, offsets, dst, dst_len, H_ED448_SCALAR, out57);
 }
 #endif

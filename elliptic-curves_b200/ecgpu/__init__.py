@@ -65,6 +65,7 @@ EXPORTS = [
     "ecg_x448_batch", "ecg_ed448_verify_batch", "ecg_ed448_mul_batch", "ecg_ed448_mul_gen_batch", "ecg_ed448_lincomb",
     "ecg_decaf448_mul_batch", "ecg_decaf448_mul_gen_batch", "ecg_decaf448_lincomb", "ecg_decaf448_check_batch",
     "ecg_decaf448_hash_to_curve_batch", "ecg_decaf448_hash_to_scalar_batch",
+    "ecg_ed448_hash_to_curve_batch", "ecg_ed448_hash_to_scalar_batch",
 ]
 
 
@@ -160,6 +161,10 @@ def load_library(path: Optional[str] = None) -> ctypes.CDLL:
     lib.ecg_ed448_mul_gen_batch.restype = ctypes.c_int
     lib.ecg_ed448_lincomb.argtypes = [vp, sz, u8p, u8p, u8p]
     lib.ecg_ed448_lincomb.restype = ctypes.c_int
+    lib.ecg_ed448_hash_to_curve_batch.argtypes = [vp, sz, u8p, u8p, u8p, sz, ctypes.c_int, u8p]
+    lib.ecg_ed448_hash_to_curve_batch.restype = ctypes.c_int
+    lib.ecg_ed448_hash_to_scalar_batch.argtypes = [vp, sz, u8p, u8p, u8p, sz, u8p]
+    lib.ecg_ed448_hash_to_scalar_batch.restype = ctypes.c_int
     lib.ecg_decaf448_mul_batch.argtypes = [vp, sz, u8p, u8p, u8p]
     lib.ecg_decaf448_mul_gen_batch.argtypes = [vp, sz, u8p, u8p]
     lib.ecg_decaf448_lincomb.argtypes = [vp, sz, u8p, u8p, u8p]
@@ -604,6 +609,37 @@ class Engine:
         self._check(self.lib.ecg_ed448_lincomb(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out)))
         return out
 
+    def ed448_hash_to_curve(self, msgs, dst: bytes, nonuniform: bool = False):
+        """Ed448 hash_from_bytes (RO) / encode_from_bytes (NU) with ExpandMsgXof<Shake256> -> n x 57 compressed records,
+        valid P57 inputs of ed448_mul"""
+        data, offs = self._pack_messages(msgs)
+        return self.ed448_hash_to_curve_packed(data, offs, dst, nonuniform)
+
+    def ed448_hash_to_curve_packed(self, data, offsets, dst: bytes, nonuniform: bool = False, out=None):
+        """the same over messages already laid out as the C ABI takes them (data + n + 1 uint64 offsets)"""
+        offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = offs.size - 1
+        if n < 0 or int(offs[-1]) > np.asarray(data).size:
+            raise ValueError("offsets: n + 1 ascending byte offsets into data")
+        data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+        if data.size == 0:
+            data = np.zeros(1, np.uint8)
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        out = _out(out, 57 * n, "out")
+        self._check(self.lib.ecg_ed448_hash_to_curve_batch(self._ctx, n, _ptr(data), _ptr(offs), _ptr(d), len(dst), 1 if nonuniform else 0,
+                                                           _ptr(out)))
+        return out.reshape(n, 57)
+
+    def ed448_hash_to_scalar(self, msgs, dst: bytes):
+        """hash_to_scalar::<Ed448, ExpandMsgXof<Shake256>, U84> over a batch -> n x 57 scalar records (byte 56 = 0), valid
+        k57 inputs of the Ed448 group entries"""
+        n = len(msgs)
+        data, offs = self._pack_messages(msgs)
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        out = np.empty(57 * n, np.uint8)
+        self._check(self.lib.ecg_ed448_hash_to_scalar_batch(self._ctx, n, _ptr(data), _ptr(offs), _ptr(d), len(dst), _ptr(out)))
+        return out.reshape(n, 57)
+
     def decaf448_mul(self, k56, P56, out=None):
         """Decaf448: out[i] = [k[i]] P[i] (n x 56 encodings; DecafPoint * DecafScalar).  Scalars are 56-byte little-endian,
         accepted iff DecafScalar::from_canonical_bytes accepts them (ScalarRangeError with the smallest index otherwise);
@@ -719,6 +755,18 @@ class Engine:
     def ed448_lincomb_ptr(self, n, k57, P57, out57):
         """ecg_ed448_lincomb on device buffers (out57: 57 bytes)"""
         self._check(self.lib.ecg_ed448_lincomb(self._ctx, n, _ptr(k57), _ptr(P57), _ptr(out57)))
+
+    def ed448_hash_to_curve_ptr(self, n, msgs, offsets, out57, dst: bytes, nonuniform: bool = False):
+        """ecg_ed448_hash_to_curve_batch on device buffers (offsets: n + 1 uint64, 8-byte aligned; records at any alignment);
+        the DST is host bytes"""
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        self._check(self.lib.ecg_ed448_hash_to_curve_batch(self._ctx, n, _ptr(msgs), _ptr(offsets), _ptr(d), len(dst), 1 if nonuniform else 0,
+                                                           _ptr(out57)))
+
+    def ed448_hash_to_scalar_ptr(self, n, msgs, offsets, out57, dst: bytes):
+        """ecg_ed448_hash_to_scalar_batch on device buffers; the DST is host bytes"""
+        d = np.frombuffer(bytes(dst), np.uint8).copy() if len(dst) else np.zeros(1, np.uint8)
+        self._check(self.lib.ecg_ed448_hash_to_scalar_batch(self._ctx, n, _ptr(msgs), _ptr(offsets), _ptr(d), len(dst), _ptr(out57)))
 
     def decaf448_mul_ptr(self, n, k56, P56, out56):
         """ecg_decaf448_mul_batch on device buffers (56-byte records, 4-byte aligned)"""

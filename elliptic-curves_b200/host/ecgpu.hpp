@@ -15,6 +15,8 @@
 //   Engine::ed448_verify(pk, sig, msgs, ctx, ph)      <->  ed448 VerifyingKey::verify_raw / verify_ctx / verify_prehashed
 //   Engine::ed448_mul / ed448_mul_gen / ed448_lincomb <->  EdwardsPoint * EdwardsScalar, Group::mul_by_generator,
 //                                                         LinearCombination::lincomb (ed448-goldilocks/src/edwards/extended.rs)
+//   Engine::ed448_hash_to_curve / ed448_hash_to_scalar <-> GroupDigest for Ed448 (hash_from_bytes / encode_from_bytes),
+//                                                         hash_to_scalar::<Ed448, ExpandMsgXof<Shake256>, U84>
 //   Engine::decaf448_mul / decaf448_mul_gen / decaf448_lincomb / decaf448_check / decaf448_hash_to_curve /
 //   decaf448_hash_to_scalar                          <->  DecafPoint * DecafScalar, GENERATOR * k, LinearCombination,
 //                                                         CompressedDecaf::decompress, GroupDigest / hash_to_scalar for Decaf448
@@ -199,6 +201,26 @@ class Engine {
     check_sizes(k.size(), P.size());
     Ed448Point out{};
     check(ecg_ed448_lincomb(ctx_, k.size(), reinterpret_cast<const uint8_t*>(k.data()), reinterpret_cast<const uint8_t*>(P.data()), out.data()));
+    return out;
+  }
+  // hash_from_bytes (nonuniform = false) / encode_from_bytes for edwards448_XOF:SHAKE256_ELL2_{RO,NU}_ under one DST:
+  // compressed points, valid inputs of ed448_mul
+  std::vector<Ed448Point> ed448_hash_to_curve(const std::vector<std::vector<uint8_t>>& msgs, const std::vector<uint8_t>& dst,
+                                              bool nonuniform = false) {
+    std::vector<uint64_t> offsets;
+    std::vector<uint8_t> data = pack(msgs, offsets);
+    std::vector<Ed448Point> out(msgs.size());
+    check(ecg_ed448_hash_to_curve_batch(ctx_, msgs.size(), data.empty() ? nullptr : data.data(), offsets.data(), dst.data(), dst.size(),
+                                        nonuniform ? 1 : 0, reinterpret_cast<uint8_t*>(out.data())));
+    return out;
+  }
+  // hash_to_scalar::<Ed448, ExpandMsgXof<Shake256>, U84>: 57-byte scalar records (byte 56 = 0)
+  std::vector<Ed448Scalar> ed448_hash_to_scalar(const std::vector<std::vector<uint8_t>>& msgs, const std::vector<uint8_t>& dst) {
+    std::vector<uint64_t> offsets;
+    std::vector<uint8_t> data = pack(msgs, offsets);
+    std::vector<Ed448Scalar> out(msgs.size());
+    check(ecg_ed448_hash_to_scalar_batch(ctx_, msgs.size(), data.empty() ? nullptr : data.data(), offsets.data(), dst.data(), dst.size(),
+                                         reinterpret_cast<uint8_t*>(out.data())));
     return out;
   }
 

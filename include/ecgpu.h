@@ -339,6 +339,30 @@ ecg_status ecg_ed448_mul_gen_batch(ecg_ctx* ctx, size_t n, const uint8_t* k57, u
  * extended.rs:310-312, the reference's default sum of products), one 57-byte record; n = 0 writes the identity. */
 ecg_status ecg_ed448_lincomb(ecg_ctx* ctx, size_t n, const uint8_t* k57, const uint8_t* P57, uint8_t out57[57]);
 
+/* Hash to curve for edwards448_XOF:SHAKE256_ELL2_RO_ / _NU_ (GroupDigest for Ed448, ed448-goldilocks/src/lib.rs:123-128)
+ * with ExpandMsgXof<Shake256>: message i = msgs[offsets[i] .. offsets[i+1]) (as in ecg_decaf448_hash_to_curve_batch),
+ * one DST for the call (host pointer; empty: ECG_EINVAL at any n; over 255 bytes: replaced by
+ * SHAKE256("H2C-OVERSIZE-DST-" || DST, 56)).  nonuniform = 0: hash_from_bytes, expand_message_xof to 2 x 84 bytes,
+ * each block read big-endian mod p (field/element.rs:76-91) through map_to_curve_elligator2, the 4-isogeny and
+ * to_edwards, the two points added, then clear_cofactor (double twice); != 0: encode_from_bytes, 84 bytes, one map.
+ * out57[i] = AffinePoint::compress of the result, the Ed448 group entries' record: it is a valid P57 input of
+ * ecg_ed448_mul_batch.  The reference's quirk is kept: u in {0, 1, p - 1} maps to (0, 0) on edwards448 (not a curve
+ * point, not the identity), which compresses to 57 zero bytes, in NU and in RO when either u is one of them; no message
+ * is known to reach these u (its 84 expanded bytes would have to be 0 or +-1 mod p).
+ * Errors: ECG_EINVAL (null ctx; empty DST; null offsets or out57 with n > 0; decreasing offsets; a null msgs with a
+ * non-empty message) and CUDA errors.  With ECG_FLAG_DEVICE_PTRS msgs, offsets and out57 are device pointers: messages
+ * and records bytewise at any alignment, offsets 8-byte aligned.  ECG_FLAG_ZEROIZE scrubs the staged messages, the
+ * intermediate points and the normalisation scratch; ECG_FLAG_CONSTTIME changes nothing (the path is branch-free).
+ * A multi-device ctx splits the batch into contiguous index ranges. */
+ecg_status ecg_ed448_hash_to_curve_batch(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets,
+                                         const uint8_t* dst, size_t dst_len, int nonuniform, uint8_t* out57);
+
+/* out57[i] = hash_to_scalar::<Ed448, ExpandMsgXof<Shake256>, U84>: 84 expanded bytes read big-endian, reduced mod ell
+ * (edwards/scalar.rs:75-89), as the 57-byte EdwardsScalar record (little-endian, byte 56 = 0): a valid k57 input of the
+ * Ed448 group entries.  Messages, DST, errors and flags as above. */
+ecg_status ecg_ed448_hash_to_scalar_batch(ecg_ctx* ctx, size_t n, const uint8_t* msgs, const uint64_t* offsets,
+                                          const uint8_t* dst, size_t dst_len, uint8_t* out57);
+
 /* ---- Decaf448 (RFC 9496): the prime-order group of ed448-goldilocks (DecafPoint, CompressedDecaf, DecafScalar) --------
  * Records: a scalar is 56 bytes little-endian (DecafScalarBytes), accepted iff DecafScalar::from_canonical_bytes
  * accepts it (ed448-goldilocks/src/decaf/scalar.rs:22-32): byte 55 >> 6 == 0 and the value is < ell, else
@@ -389,7 +413,7 @@ ecg_status ecg_microbench(ecg_ctx* ctx, int which, int iters, double* ops_per_s,
 
 /* When enabled, every call brackets its dominant kernel (variable-base / fixed-base scalar multiplication, the X448 ladder,
  * the Ed448 verification kernel, the Ed448 and Decaf448 scalar-multiplication kernels, the Decaf448 check and hash
- * kernels)
+ * kernels, the Ed448 hash kernels)
  * with CUDA events on the launching stream; ecg_timing_read returns the accumulated device milliseconds
  * (max over the ctx's devices per call) and the number of calls since ecg_timing_enable. */
 ecg_status ecg_timing_enable(ecg_ctx* ctx, int on);

@@ -117,6 +117,14 @@ unsafe extern "C" {
     /// `hash_to_scalar::<Decaf448, ExpandMsgXof<Shake256>, U64>` over a batch (56-byte little-endian scalars)
     pub fn ecg_decaf448_hash_to_scalar_batch(ctx: *mut ecg_ctx, n: usize, msgs: *const u8, offsets: *const u64, dst: *const u8,
                                              dst_len: usize, out56: *mut u8) -> i32;
+    /// Ed448 `hash_from_bytes` (nonuniform = 0) / `encode_from_bytes` with `ExpandMsgXof<Shake256>`
+    /// (edwards448_XOF:SHAKE256_ELL2_RO_ / _NU_); message i = `msgs[offsets[i]..offsets[i + 1]]`, one DST; 57-byte
+    /// compressed records
+    pub fn ecg_ed448_hash_to_curve_batch(ctx: *mut ecg_ctx, n: usize, msgs: *const u8, offsets: *const u64, dst: *const u8,
+                                         dst_len: usize, nonuniform: i32, out57: *mut u8) -> i32;
+    /// `hash_to_scalar::<Ed448, ExpandMsgXof<Shake256>, U84>` over a batch (57-byte scalar records, byte 56 = 0)
+    pub fn ecg_ed448_hash_to_scalar_batch(ctx: *mut ecg_ctx, n: usize, msgs: *const u8, offsets: *const u64, dst: *const u8,
+                                          dst_len: usize, out57: *mut u8) -> i32;
     pub fn ecg_kernel_launches(ctx: *const ecg_ctx) -> u64;
 }
 
@@ -281,6 +289,31 @@ impl GpuEngine {
             } else {
                 ecg_decaf448_hash_to_curve_batch(self.ctx, n, data_ptr, offsets.as_ptr(), dst.as_ptr(), dst.len(), nonuniform as i32,
                                                  out.as_mut_ptr().cast())
+            }
+        };
+        self.check(rc).map(|_| out)
+    }
+
+    /// Ed448 hash to curve (`hash_from_bytes`, or `encode_from_bytes` with `nonuniform`) or, with `scalar`,
+    /// `hash_to_scalar` under one DST: one 57-byte record per message, the input format of `batch_mul_ed448`
+    pub fn batch_hash_ed448(&mut self, msgs: &[&[u8]], dst: &[u8], nonuniform: bool, scalar: bool) -> Result<Vec<[u8; 57]>, GpuError> {
+        let n = msgs.len();
+        let mut offsets = Vec::with_capacity(n + 1);
+        let mut data = Vec::new();
+        offsets.push(0u64);
+        for m in msgs {
+            data.extend_from_slice(m);
+            offsets.push(data.len() as u64);
+        }
+        let mut out = vec![[0u8; 57]; n];
+        let data_ptr = if data.is_empty() { core::ptr::null() } else { data.as_ptr() };
+        // SAFETY: offsets holds n + 1 entries into data, dst dst.len() bytes, out n records of 57 bytes.
+        let rc = unsafe {
+            if scalar {
+                ecg_ed448_hash_to_scalar_batch(self.ctx, n, data_ptr, offsets.as_ptr(), dst.as_ptr(), dst.len(), out.as_mut_ptr().cast())
+            } else {
+                ecg_ed448_hash_to_curve_batch(self.ctx, n, data_ptr, offsets.as_ptr(), dst.as_ptr(), dst.len(), nonuniform as i32,
+                                              out.as_mut_ptr().cast())
             }
         };
         self.check(rc).map(|_| out)

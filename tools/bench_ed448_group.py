@@ -1,8 +1,10 @@
 #!/usr/bin/env python3
-"""Ed448 group-operation throughput of ecg_ed448_mul_batch (k P), ecg_ed448_mul_gen_batch (k B) and ecg_ed448_lincomb
-on one GPU; prints one JSON line.
+"""Ed448 group-operation throughput of ecg_ed448_mul_batch (k P), ecg_ed448_mul_gen_batch (k B) and ecg_ed448_lincomb,
+and of hashing with ecg_ed448_hash_to_curve_batch (RO, NU) and ecg_ed448_hash_to_scalar_batch, on one GPU; prints one
+JSON line.
 
-    python tools/bench_ed448_group.py [--n-mul 1048576] [--n-gen 4194304] [--n-lin 1048576] [--steps 5] [--warmup 2]
+    python tools/bench_ed448_group.py [--n-mul 1048576] [--n-gen 4194304] [--n-lin 1048576] [--n-hash 4194304]
+                                      [--steps 5] [--warmup 2] [--hash-only]
 
 The workload: secret scalars a(s) = clamp(SHAKE256(s)[:57]) mod ell of random seeds s, with OpenSSL's public keys
 pub(s) = [a(s)]B, 1,024 of them as the points of k P and of the linear combination; random scalars k < ell.
@@ -15,6 +17,10 @@ Per entry (mul, mul_gen, lincomb):
 - <entry>_bit_exact: mul_gen: every output of the last step against OpenSSL's public keys; mul: every output of the
   last step against mul_gen(k a(s) mod ell) (the identity [k]([a]B) = [k a]B) and a sample against the Python model;
   lincomb: against mul_gen(sum k_i a_i mod ell) and the model's sum over the first terms.
+Per hashing entry (h2c_ro, h2c_nu, h2s): 32-byte random messages, device-resident (messages, offsets and records), one
+DST; <entry>_per_s end to end (the hash kernel and, for points, the normalisation kernel), <entry>_kernel_ms the hash
+kernel alone, <entry>_imad_fraction its cost-model count at its rate against ecg_microbench(0), <entry>_bit_exact a
+sample of the last step against the Python model (tests/ed448_h2c_model.py).  --hash-only runs these alone.
 CPU baselines on the host cores: OpenSSL Ed448 key generation (a k B per key) and OpenSSL X448 (the same-size ladder on
 the isogenous Montgomery curve) for the variable base.  There is no CPU fallback: without a CUDA device the script fails."""
 import argparse
@@ -43,6 +49,18 @@ VARBASE = (M14 + 4 * M14 + 4 * S14 + 7 * 9 * M14 + 9 * SMALL) + 444 * (3 * M14 +
 FIXED = 56 * 8 * M14
 NORM = 5 * M14 + (453 * S14 + 13 * M14) // 32
 IMAD = {"mul": DECOMP + VARBASE + NORM, "mul_gen": FIXED + NORM, "lincomb": DECOMP + VARBASE + 9 * M14 + SMALL}
+# hashing (ecg_ed448_h2c.cuh; estimates from the code, not measurements; Keccak runs on the ALU pipe and is not counted):
+#   the inverse-square-root chain (p - 3) / 4: 451 S + 12 M;
+#   one map with the homogenised isogeny: the chain + 18 M + 8 S + 7 small;
+#   RO kernel: two maps, one addition (9 M + 1 small), two doublings (3 M + 4 S, then 4 M + 4 S); NU kernel: one map and
+#   the doublings; both then pay the normalisation's share NORM;
+#   hash to scalar: the 6 folds of 17 x 7 products of the 114-byte reduction mod ell.
+ISR = 451 * S14 + 12 * M14
+MAP = ISR + 18 * M14 + 8 * S14 + 7 * SMALL
+DBL2 = 7 * M14 + 8 * S14
+H2C_KERNEL = {"h2c_ro": 2 * MAP + 9 * M14 + SMALL + DBL2, "h2c_nu": MAP + DBL2, "h2s": 6 * 17 * 7}
+IMAD.update({"h2c_ro": H2C_KERNEL["h2c_ro"] + NORM, "h2c_nu": H2C_KERNEL["h2c_nu"] + NORM, "h2s": H2C_KERNEL["h2s"]})
+H2C_DST = b"edwards448_XOF:SHAKE256_ELL2_RO_"
 L = 2**446 - 13818066809895115352007386748515426880336692474882178609894547503885
 NPOINTS = 1024
 
@@ -125,6 +143,47 @@ def time_host(call, steps):
     return float(np.median(t))
 
 
+def bench_hash(a):
+    """the hashing entries on n 32-byte messages, device-resident end to end"""
+    import torch
+
+    import ecgpu
+    import ed448_h2c_model as H
+
+    n = a.n_hash
+    rng = np.random.default_rng(9380)
+    data = rng.integers(0, 256, 32 * n, dtype=np.uint8)
+    offs = np.arange(0, 32 * (n + 1), 32, dtype=np.uint64)
+    eng = ecgpu.Engine([0], device_ptrs=True)
+    peak, _ = eng.microbench(0)
+    rec = {"n_hash": n, "hash_msg_bytes": 32, "hash_imad_peak_per_s": peak}
+    dd, do = torch.from_numpy(data).cuda(), torch.from_numpy(offs.view(np.int64)).cuda()
+    od = torch.empty(57 * n, dtype=torch.uint8, device="cuda")
+    calls = {"h2c_ro": lambda: eng.ed448_hash_to_curve_ptr(n, dd.data_ptr(), do.data_ptr(), od.data_ptr(), H2C_DST, False),
+             "h2c_nu": lambda: eng.ed448_hash_to_curve_ptr(n, dd.data_ptr(), do.data_ptr(), od.data_ptr(), H2C_DST, True),
+             "h2s": lambda: eng.ed448_hash_to_scalar_ptr(n, dd.data_ptr(), do.data_ptr(), od.data_ptr(), H2C_DST)}
+    models = {"h2c_ro": lambda m: H.hash_to_curve(m, H2C_DST), "h2c_nu": lambda m: H.hash_to_curve(m, H2C_DST, True),
+              "h2s": lambda m: H.hash_to_scalar(m, H2C_DST)}
+    ok_all = True
+    for name, call in calls.items():
+        ms, kms = time_device(eng, call, a.steps, a.warmup)
+        got = od.cpu().numpy()
+        idx = sorted(set(np.linspace(0, n - 1, min(n, a.model_checked)).astype(int).tolist()))
+        ok = all(bytes(got[57 * i:57 * i + 57]) == models[name](bytes(data[32 * i:32 * i + 32])) for i in idx)
+        ok_all = ok_all and ok
+        rec[f"{name}_per_s"] = n / (ms * 1e-3)
+        rec[f"{name}_step_ms"] = ms
+        rec[f"{name}_kernel_ms"] = kms
+        rec[f"{name}_imad_per_elem"] = IMAD[name]
+        rec[f"{name}_kernel_imad_per_elem"] = H2C_KERNEL[name]
+        rec[f"{name}_imad_fraction"] = n / (kms * 1e-3) * H2C_KERNEL[name] / peak
+        rec[f"{name}_bit_exact"] = ok
+    rec["hash_model_checked"] = len(idx)
+    rec["hash_bit_exact"] = ok_all
+    eng.close()
+    return rec
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n-mul", type=int, default=1 << 20)
@@ -133,6 +192,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--model-checked", type=int, default=256)
+    ap.add_argument("--n-hash", type=int, default=1 << 22)
+    ap.add_argument("--hash-only", action="store_true")
     a = ap.parse_args()
     import torch
 
@@ -143,6 +204,11 @@ def main():
 
     if not torch.cuda.is_available():
         sys.exit("bench_ed448_group: no CUDA device (there is no CPU fallback)")
+    if a.hash_only:
+        rec = {"metric": "ed448_hash_per_s", "steps": a.steps, "warmup": a.warmup, **gpu_info()}
+        rec.update(bench_hash(a))
+        print(json.dumps(rec))
+        return
     procs = os.cpu_count() or 1
     rng = np.random.default_rng(448)
     ngen = a.n_gen
@@ -225,6 +291,8 @@ def main():
     rec["cpu_baseline_openssl_x448_per_s"] = cpu_rate(_x448_chunk, 2000, procs)
     rec["speedup_mul_gen_vs_openssl_keygen"] = rec["mul_gen_per_s"] / rec["cpu_baseline_openssl_ed448_keygen_per_s"]
     rec["speedup_mul_vs_openssl_x448"] = rec["mul_per_s"] / rec["cpu_baseline_openssl_x448_per_s"]
+    rec.update(bench_hash(a))
+    rec["bit_exact"] = rec["bit_exact"] and rec["hash_bit_exact"]
     print(json.dumps(rec))
 
 
